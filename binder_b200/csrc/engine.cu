@@ -867,7 +867,10 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     P.epoch = (uint32_t)(++e->epoch);
     P.stage_log = e->stage_log;
     P.n_dev = nullptr; P.qidx_map = nullptr; P.route = 0; P.nranks = 1; P.rank = 0; P.regions = 0; P.bounce = bounce; P.qidx_out = nullptr; P.err_in = nullptr; P.tcp = (flags & BB_BATCH_TCP) ? 1u : 0u;
-    if (n == 0) { CK(cudaMemsetAsync(d_out_off, 0, 4, st)); CK(cudaMemsetAsync(d_totals, 0, 16, st)); return BB_OK; }
+    // An empty batch still runs one block: its last-block path writes out_off[0] = 0 and totals {0, 0, -, epoch}, so a
+    // caller polling the done marker sees this launch finish like any other (no tiles, so nothing to stamp)
+    if (n == 0) P.stage_log = nullptr;
+    const uint32_t grid = P.ntiles ? P.ntiles : 1u;
     // Which variant: the service variant (copy jobs + emit rounds, a tile per SM fewer) pays off when answers are long.  Decided
     // from the latest batch whose totals are known: the host path learns them in bb_resolve_wait, the device path from a
     // 16-byte copy of d_totals that follows every launch (looked at only once its epoch has landed: no synchronisation).
@@ -885,11 +888,11 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     P.fb = (feedback && e->profile == 0) ? e->h_fb + 4 * (P.epoch % bb_engine::FB) : nullptr;
     // no memsets: the kernel leaves desc/counter zeroed for the next launch (self-cleaning)
     if (svc) {
-        if (e->ordered) bbk::resolve_kernel<true, false, true><<<P.ntiles, bbk::T, 0, st>>>(P);
-        else bbk::resolve_kernel<false, false, true><<<P.ntiles, bbk::T, 0, st>>>(P);
+        if (e->ordered) bbk::resolve_kernel<true, false, true><<<grid, bbk::T, 0, st>>>(P);
+        else bbk::resolve_kernel<false, false, true><<<grid, bbk::T, 0, st>>>(P);
     } else {
-        if (e->ordered) bbk::resolve_kernel<true, false, false><<<P.ntiles, bbk::T, 0, st>>>(P);
-        else bbk::resolve_kernel<false, false, false><<<P.ntiles, bbk::T, 0, st>>>(P);
+        if (e->ordered) bbk::resolve_kernel<true, false, false><<<grid, bbk::T, 0, st>>>(P);
+        else bbk::resolve_kernel<false, false, false><<<grid, bbk::T, 0, st>>>(P);
     }
     CK(cudaGetLastError());
     e->launches++;
@@ -936,8 +939,9 @@ int bb_resolve_submit_ex(bb_engine* e, int slot, const uint8_t* pkts, const uint
     // kernel's coalesced flush writes the responses straight into it over PCIe: no device staging, no
     // D2H copies and no host round trip to learn the sizes.  Otherwise: staged copies (below).
     const void* outs[5] = { out, out_off, out_len, status, miss_idx };
+    // (whether the set is pinned does not depend on n: an empty batch must not cache "not pinned" for its buffers)
     if (memcmp(outs, s.zc_seen, sizeof outs) != 0) {
-        bool ok = n != 0 && (((uintptr_t)out & 15) == 0);
+        bool ok = ((uintptr_t)out & 15) == 0;
         for (int i = 0; ok && i < 5; i++) {
             cudaPointerAttributes at;
             ok = cudaPointerGetAttributes(&at, outs[i]) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer == outs[i];

@@ -412,7 +412,8 @@ struct Query {
 };
 
 bool decode(const uint8_t* p, uint32_t len, Query& q) {
-    if (len < 12) return false;
+    // a DNS message is at most 65,535 bytes (RFC 1035 4.2.2 framing; the engine's u16 response length): anything longer is not a query
+    if (len < 12 || len > 65535) return false;
     q.pkt = p; q.len = len;
     q.id = (uint16_t)(p[0] << 8 | p[1]);
     if (p[2] & 0x80) return false;                        // QR=1: not a query

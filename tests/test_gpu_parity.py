@@ -16,8 +16,15 @@ from binder_b200.engine import repack
 def assert_same(gpu, orc, data, off, seed=0, qidx_base=0, **kw):
     """GPU result == oracle result: status, every response's bytes, the miss set — and in
     ordered mode also the exact layout (offsets, packed bytes, ascending miss list)."""
-    out, ooff, olen, status, miss = gpu.resolve_batch(data, off, seed=seed, qidx_base=qidx_base, **kw)
-    o_out, o_off, o_len, o_status, o_miss = orc.resolve_batch(data, off, seed=seed, qidx_base=qidx_base, **kw)
+    return compare(gpu.resolve_batch(data, off, seed=seed, qidx_base=qidx_base, **kw),
+                   orc.resolve_batch(data, off, seed=seed, qidx_base=qidx_base, **kw), data, off, gpu.ordered)
+
+
+def compare(res, oracle_res, data, off, ordered):
+    """The checks of assert_same on results already computed: res = (out, out_off, out_len, status, miss) from the
+    engine, oracle_res the same from the oracle; ordered = the engine's packing."""
+    out, ooff, olen, status, miss = res
+    o_out, o_off, o_len, o_status, o_miss = oracle_res
     n = len(off) - 1
     bad = np.nonzero(status != o_status)[0]
     assert bad.size == 0, ('status differs at', bad[:5], status[bad[:5]], o_status[bad[:5]])
@@ -30,7 +37,7 @@ def assert_same(gpu, orc, data, off, seed=0, qidx_base=0, **kw):
                 q = bytes(data[off[i]:off[i + 1]])
                 raise AssertionError('query %d %r\n gpu    %s\n oracle %s' % (i, q, a.hex(), b.hex()))
         raise AssertionError('length arrays differ')
-    if gpu.ordered:
+    if ordered:
         assert np.array_equal(ooff, o_off) and np.array_equal(out, o_out) and np.array_equal(miss, o_miss)
     else:
         # arrival packing: a permutation of whole responses, no gaps, no overlap
@@ -82,15 +89,13 @@ def test_batch_size_edges(n, ordered):
     assert_same(gpu, orc, data, off, seed=99)
 
 
-@pytest.mark.parametrize('ordered', MODES)
-def test_tiles_larger_than_staging(ordered):
-    """Tiles whose packets (> 8 KB) or responses (> 12 KB) exceed the shared-memory staging."""
+def staging_case():
+    """(snapshot, packets): tiles whose packets (> 8 KB) or responses (> 12 KB) exceed the shared-memory staging."""
     kids = [('/com/foo/svc/lb%02d' % i, {'type': 'load_balancer', 'load_balancer': {'address': '10.0.0.%d' % i}})
             for i in range(30)]
     snap = H.snapshot([('/com/foo', None), ('/com/foo/svc', {'type': 'service', 'service': {
         'srvce': '_http', 'proto': '_tcp', 'port': 80}})] + kids +
         [('/com/foo/' + 'h' * 60, {'type': 'host', 'host': {'address': '10.9.9.9'}})])
-    gpu, orc = pair('foo.com', snap, ordered=ordered)
     big = synth.make_query('_http._tcp.svc.foo.com', 'SRV', edns=4096) + b'\x55' * 200
     long_a = synth.make_query('H' * 60 + '.foo.com', 'A', edns=1232)
     pkts = []
@@ -100,6 +105,14 @@ def test_tiles_larger_than_staging(ordered):
             pkts.append(synth.make_query('svc.foo.com', 'A'))
         if i % 11 == 0:
             pkts.append(b'\x00' * 5)
+    return snap, pkts
+
+
+@pytest.mark.parametrize('ordered', MODES)
+def test_tiles_larger_than_staging(ordered):
+    """Tiles whose packets (> 8 KB) or responses (> 12 KB) exceed the shared-memory staging."""
+    snap, pkts = staging_case()
+    gpu, orc = pair('foo.com', snap, ordered=ordered)
     data, off = synth.pack_batch(pkts)
     assert_same(gpu, orc, data, off, seed=4242)
 

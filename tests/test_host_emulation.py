@@ -172,6 +172,36 @@ def test_emulated_sharded_pipeline(L, seed, world):
     assert seen == n
 
 
+def padded_queries(lengths):
+    """A valid query padded with trailing bytes to each length (and a short query after each): a DNS message is at
+    most 65,535 bytes, so the padded ones up to that are answered and the longer ones are dropped."""
+    pk = []
+    for i, ln in enumerate(lengths):
+        q = synth.make_query('hosta.foo.com' if i % 2 == 0 else '_http._tcp.svc.foo.com', 'A' if i % 2 == 0 else 'SRV', qid=i)
+        pk += [q + bytes([0x41 + i % 7]) * (ln - len(q)), synth.make_query('hostb.foo.com', 'A', qid=1000 + i)]
+    return pk
+
+
+def size_zone():
+    return H.snapshot([('/com/foo', None), ('/com/foo/hosta', {'type': 'host', 'host': {'address': '10.0.0.1'}}),
+                       ('/com/foo/hostb', {'type': 'host', 'host': {'address': '10.0.0.2'}}),
+                       ('/com/foo/svc', {'type': 'service', 'service': {'srvce': '_http', 'proto': '_tcp', 'port': 80}}),
+                       ('/com/foo/svc/lb0', {'type': 'load_balancer', 'load_balancer': {'address': '10.1.0.1'}})])
+
+
+@pytest.mark.parametrize('tcp', [False, True], ids=['udp', 'tcp'])
+def test_emulated_packet_length_limit(L, tcp):
+    """Packets of 65,534 and 65,535 bytes are queries (trailing bytes ignored); 65,536 and 70,000 bytes are dropped,
+    by the device code and the oracle alike."""
+    snap = size_zone()
+    emu = EmuEngine(L, 'foo.com', snap)
+    orc = H.make_impl('oracle', 'foo.com', snap)
+    lengths = [65534, 65535, 65536, 70000, 65535, 70000]
+    data, off = synth.pack_batch(padded_queries(lengths))
+    g = assert_same(emu, orc, data, off, seed=5, tcp=tcp)
+    assert list(g[3][0::2]) == [0, 0, 2, 2, 0, 2] and (g[3][1::2] == 0).all()
+
+
 def _path_counts(L, reset=True):
     c = (ctypes.c_ulonglong * 2)()
     L.bb_emu_path_counts(c, int(reset))

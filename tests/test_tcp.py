@@ -131,13 +131,9 @@ def test_tcp_server_gpu():
     _serve_and_check('gpu')
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize('ordered', [False, True])
-def test_gpu_tcp_batches_are_bit_exact(ordered):
-    from test_gpu_parity import assert_same
-    snap = big_zone()
-    gpu = H.make_impl('gpu', 'foo.com', snap, ordered=ordered)
-    orc = H.make_impl('oracle', 'foo.com', snap)
+def big_zone_batch():
+    """700 queries on big_zone(): the 200- and 1,300-child services (answers of up to 65,535 bytes over TCP) among
+    short answers, misses and NOTIMP."""
     rng = random.Random(8)
     pk = []
     for i in range(700):
@@ -152,7 +148,17 @@ def test_gpu_tcp_batches_are_bit_exact(ordered):
             pk.append(synth.make_query('huge.foo.com', 'A', qid=i))
         else:
             pk.append(synth.make_query(rng.choice(['hosta.foo.com', 'nope.foo.com', 'lb007.big.foo.com']), rng.choice(['A', 'SRV', 'AAAA']), qid=i))
-    data, off = synth.pack_batch(pk)
+    return pk
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize('ordered', [False, True])
+def test_gpu_tcp_batches_are_bit_exact(ordered):
+    from test_gpu_parity import assert_same
+    snap = big_zone()
+    gpu = H.make_impl('gpu', 'foo.com', snap, ordered=ordered)
+    orc = H.make_impl('oracle', 'foo.com', snap)
+    data, off = synth.pack_batch(big_zone_batch())
     assert_same(gpu, orc, data, off, seed=77, tcp=True)
     assert_same(gpu, orc, data, off, seed=77)                   # and the same engine still applies the UDP limits
 
