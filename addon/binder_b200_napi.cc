@@ -145,6 +145,43 @@ static napi_value ResolveBatch(napi_env env, napi_callback_info info) {
     return res;
 }
 
+// relayBatch(engine, pkts: Buffer, pktOff: Uint32Array(n+1), upstream: Buffer, upOff: Uint32Array(n+1)[, tcp: boolean])
+//   -> {out, outOff, outLen, status}: the replies Recursion.prototype.resolve's respond() builds from the upstream's
+//   answers (lib/recursion.js:287-327, bb_relay_batch); an empty upstream (upOff[i] == upOff[i+1]) = the lookup failed
+static bool check_off(napi_env env, napi_value v, size_t bytes, const uint32_t** off, size_t* n) {
+    napi_typedarray_type tt; void* p; napi_value ab; size_t bo;
+    if (napi_get_typedarray_info(env, v, &tt, n, &p, &ab, &bo) != napi_ok || tt != napi_uint32_array || *n < 1 || *n > (1u << 22) + 1) return false;
+    *off = (const uint32_t*)p;
+    for (size_t i = 1; i < *n; i++) if ((*off)[i] < (*off)[i - 1]) return false;
+    return (*off)[*n - 1] <= bytes;
+}
+static napi_value RelayBatch(napi_env env, napi_callback_info info) {
+    size_t argc = 6; napi_value argv[6];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    bool tcp = false;
+    if (argc > 5) napi_get_value_bool(env, argv[5], &tcp);
+    void* e; NAPI_OK(napi_get_value_external(env, argv[0], &e));
+    void* pk; size_t pklen; NAPI_OK(napi_get_buffer_info(env, argv[1], &pk, &pklen));
+    void* up; size_t uplen; NAPI_OK(napi_get_buffer_info(env, argv[3], &up, &uplen));
+    const uint32_t *qo, *uo; size_t qn, un;
+    if (!check_off(env, argv[2], pklen, &qo, &qn) || !check_off(env, argv[4], uplen, &uo, &un) || qn != un) return Throw(env, BB_ERR_ARG);
+    const uint32_t n = (uint32_t)qn - 1;
+    const uint64_t cap64 = (uint64_t)n * (tcp ? 65535u : 1200u);
+    const uint32_t cap = cap64 > 0xFFFFFF00u ? 0xFFFFFF00u : (uint32_t)cap64;
+    void *out, *oo, *ol, *st; napi_value o_out, a_oo, a_ol, a_st, t_oo, t_ol, t_st;
+    NAPI_OK(napi_create_buffer(env, cap, &out, &o_out));
+    NAPI_OK(napi_create_arraybuffer(env, (n + 1) * 4, &oo, &a_oo)); NAPI_OK(napi_create_typedarray(env, napi_uint32_array, n + 1, a_oo, 0, &t_oo));
+    NAPI_OK(napi_create_arraybuffer(env, n * 2, &ol, &a_ol));       NAPI_OK(napi_create_typedarray(env, napi_uint16_array, n, a_ol, 0, &t_ol));
+    NAPI_OK(napi_create_arraybuffer(env, n, &st, &a_st));           NAPI_OK(napi_create_typedarray(env, napi_uint8_array, n, a_st, 0, &t_st));
+    int rc = bb_relay_batch((bb_engine*)e, (const uint8_t*)pk, qo, (const uint8_t*)up, uo, n, tcp ? BB_BATCH_TCP : 0u, (uint8_t*)out, cap,
+                            (uint32_t*)oo, (uint16_t*)ol, (uint8_t*)st);
+    if (rc != BB_OK) return Throw(env, rc);
+    napi_value res; NAPI_OK(napi_create_object(env, &res));
+    napi_set_named_property(env, res, "out", o_out);   napi_set_named_property(env, res, "outOff", t_oo);
+    napi_set_named_property(env, res, "outLen", t_ol); napi_set_named_property(env, res, "status", t_st);
+    return res;
+}
+
 static napi_value Init(napi_env env, napi_value exports) {
     napi_property_descriptor d[] = {
         { "zoneBuild", nullptr, ZoneBuild, nullptr, nullptr, nullptr, napi_default, nullptr },
@@ -154,6 +191,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         { "engineApplyUpdate", nullptr, EngineApplyUpdate, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "engineSetRecursionFilter", nullptr, EngineSetRecursionFilter, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "resolveBatch", nullptr, ResolveBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "relayBatch", nullptr, RelayBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
     };
     napi_define_properties(env, exports, sizeof d / sizeof d[0], d);
     return exports;

@@ -49,6 +49,9 @@ SYMBOLS = {
     'bb_resolve_batch_device': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint32, _c.c_uint64,
                                            _c.c_uint32, _c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p,
                                            _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p]),
+    'bb_relay_batch': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p,
+                                                      _c.c_void_p]),
+    'bb_relay_batch_device': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_uint32] + [_c.c_void_p] * 5),
     'bb_engine_launch_count': (_c.c_uint64, [_c.c_void_p]),
     'bb_engine_launch_epoch': (_c.c_uint32, [_c.c_void_p]),
     'bb_engine_set_stage_log': (None, [_c.c_void_p, _c.c_void_p]),

@@ -1,4 +1,4 @@
-// binder_b200 engine: the CUDA resolve kernel for sm_100a and the host side of the C ABI.
+// binder_b200 engine: the CUDA resolve and relay kernels for sm_90a and the host side of the C ABI.
 //
 // One kernel does the whole of binder's per-query path for a batch of raw DNS packets:
 //   mname decode                      -> decode()                 (call site lib/server.js:443-446,471)
@@ -8,6 +8,8 @@
 //   shuffle                           -> make_perm()/perm_at()    (lib/server.js:40-53)
 //   mname encode + respond            -> emit_response()          (lib/server.js:130,286,299,310,398-402,413-414,427)
 //   miss hand-off to recursion        -> compacted miss_idx[]     (lib/server.js:110-113,222-225)
+// and a second kernel turns the upstream responses to forwarded misses into binder's replies:
+//   Recursion.resolve's respond()     -> relay_kernel / relay_size() + relay_emit()   (lib/recursion.js:287-327)
 //
 // Data movement (HBM-bound integer/byte work, no tensor cores):
 //   * a CTA owns a tile of 128 consecutive queries; their packed bytes are one contiguous
@@ -22,6 +24,7 @@
 
 #include <cuda_runtime.h>
 #include <cstdio>
+#include <algorithm>
 #include <cstring>
 #include <string>
 #include <vector>
@@ -32,12 +35,52 @@ extern "C" void bb_zone_mark_synced(bb_zone* z);
 extern "C" uint64_t bb_zone_sync_gen(const bb_zone* z);
 
 #include "resolve_device.cuh"
+#include "relay_device.cuh"
 
 namespace bbk {
 // ---- the kernel ------------------------------------------------------------------------------
 __device__ __forceinline__ uint64_t warp_sum64(uint64_t v) {
     for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
     return v;
+}
+
+// Single-pass decoupled look-back (ordered packing), run by warp 0 of the tile: publishes the tile's aggregate `agg`,
+// sums its predecessors' descriptors back to the nearest inclusive prefix (a window of 128 predecessors, 4 independent
+// loads per lane), publishes its own inclusive prefix.  -> the exclusive prefix, in every lane.
+__device__ __forceinline__ uint64_t lookback(unsigned long long* desc, uint32_t tile, uint64_t agg, int lane) {
+    volatile unsigned long long* D = desc;
+    uint64_t ex = 0;
+    if (tile == 0) { if (lane == 0) D[0] = D_FLAG_P | agg; }
+    else {
+        if (lane == 0) D[tile] = D_FLAG_A | agg;
+        int base = (int)tile - 1;
+        for (;;) {
+            uint64_t d[4];
+            bool ready;
+            do {
+                ready = true;
+#pragma unroll
+                for (int k = 0; k < 4; k++) {
+                    const int idx = base - lane - 32 * k;
+                    d[k] = idx >= 0 ? D[idx] : D_FLAG_P;
+                    ready &= (d[k] >> 62) != 0;
+                }
+            } while (__any_sync(0xffffffffu, !ready));
+            uint32_t mypos = 0xFFFFFFFFu;            // distance of the nearest predecessor with an inclusive prefix
+#pragma unroll
+            for (int k = 3; k >= 0; k--) if ((d[k] >> 62) == 2) mypos = (uint32_t)(lane + 32 * k);
+            uint32_t minpos = mypos;
+            for (int o = 16; o; o >>= 1) minpos = min(minpos, __shfl_xor_sync(0xffffffffu, minpos, o));
+            uint64_t part = 0;
+#pragma unroll
+            for (int k = 0; k < 4; k++) if ((uint32_t)(lane + 32 * k) <= minpos) part += d[k] & D_VAL;
+            ex += warp_sum64(part);
+            if (minpos != 0xFFFFFFFFu) break;
+            base -= 128;
+        }
+        if (lane == 0) D[tile] = D_FLAG_P | (ex + agg);
+    }
+    return ex;
 }
 
 // ---- bulk asynchronous copies (the TMA unit's 1-D form) and the mbarrier they complete on ------------------------
@@ -228,39 +271,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
             s_prefix = atomicAdd(r_desc + P.ntiles_cap, (unsigned long long)tile_bytes | ((unsigned long long)tile_miss << D_MISS_SHIFT));
     } else
     if (warp == 0) {
-        volatile unsigned long long* D = r_desc;
-        const uint64_t agg = (uint64_t)tile_bytes | ((uint64_t)tile_miss << D_MISS_SHIFT);
-        uint64_t ex = 0;
-        if (tile == 0) { if (lane == 0) D[0] = D_FLAG_P | agg; }
-        else {
-            if (lane == 0) D[tile] = D_FLAG_A | agg;
-            int base = (int)tile - 1;
-            for (;;) {                                   // window of 128 predecessors, 4 independent loads per lane
-                uint64_t d[4];
-                bool ready;
-                do {
-                    ready = true;
-#pragma unroll
-                    for (int k = 0; k < 4; k++) {
-                        const int idx = base - lane - 32 * k;
-                        d[k] = idx >= 0 ? D[idx] : D_FLAG_P;
-                        ready &= (d[k] >> 62) != 0;
-                    }
-                } while (__any_sync(0xffffffffu, !ready));
-                uint32_t mypos = 0xFFFFFFFFu;            // distance of the nearest predecessor with an inclusive prefix
-#pragma unroll
-                for (int k = 3; k >= 0; k--) if ((d[k] >> 62) == 2) mypos = (uint32_t)(lane + 32 * k);
-                uint32_t minpos = mypos;
-                for (int o = 16; o; o >>= 1) minpos = min(minpos, __shfl_xor_sync(0xffffffffu, minpos, o));
-                uint64_t part = 0;
-#pragma unroll
-                for (int k = 0; k < 4; k++) if ((uint32_t)(lane + 32 * k) <= minpos) part += d[k] & D_VAL;
-                ex += warp_sum64(part);
-                if (minpos != 0xFFFFFFFFu) break;
-                base -= 128;
-            }
-            if (lane == 0) D[tile] = D_FLAG_P | (ex + agg);
-        }
+        const uint64_t ex = lookback(r_desc, tile, (uint64_t)tile_bytes | ((uint64_t)tile_miss << D_MISS_SHIFT), lane);
         if (lane == 0) s_prefix = ex;
     }
     __syncthreads();
@@ -431,6 +442,139 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     }
 }
 
+// ---- recursion relay (DESIGN.md section 13, lib/recursion.js:287-327) ------------------------------------------------
+// One launch per batch.  A CTA takes a tile of 128 relays, a thread per relay.  The tile's query bytes and its upstream
+// bytes are two contiguous ranges of their batches: each is staged into shared memory with one bulk copy when it fits
+// (otherwise the relays read global memory).  Then decode + sizing (relay_size), a CTA scan, placement (arrival claim, or
+// the look-back for ordered packing), and the emit (relay_emit) straight to the output — or, when the results go to
+// pinned host memory, to the device bounce buffer and from there with coalesced 16-byte stores.  Self-cleaning like
+// resolve_kernel: a step is one launch.
+constexpr int RS_Q = 8192;                // staged query bytes per tile
+constexpr int RS_UP = 24576;              // staged upstream bytes per tile
+struct RelayParams {
+    const uint8_t* q; const uint32_t* q_off; const uint8_t* up; const uint32_t* up_off; uint32_t n;
+    uint8_t* out; uint32_t out_cap; uint32_t* out_off; uint16_t* out_len; uint8_t* status; uint32_t* totals;
+    uint8_t* bounce;                      // zero-copy results: device buffer (same offsets as `out`) written first
+    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap;
+    uint32_t epoch, tcp;
+};
+// thread 0: the byte range [f0, f1) of a batch into shared memory with one bulk copy, when it fits `cap`
+__device__ __forceinline__ bool stage_fits(uint32_t f0, uint32_t f1, uint32_t cap) { return f1 >= f0 && f1 - (f0 & ~15u) <= cap; }
+__device__ __forceinline__ void stage_range(uint32_t bar, uint8_t* s, const uint8_t* g, uint32_t f0, uint32_t f1, uint32_t cap) {
+    const uint32_t fa = f0 & ~15u;
+    if (stage_fits(f0, f1, cap) && f1 > fa) {
+        const uint32_t bytes = (f1 - fa + 15) & ~15u;
+        mbar_expect_tx(bar, bytes);
+        bulk_g2s((uint32_t)__cvta_generic_to_shared(s), g + fa, bytes, bar);
+    }
+}
+
+template <bool ORDERED>
+__global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
+    __shared__ __align__(16) uint8_t s_q[RS_Q + 32];
+    __shared__ __align__(16) uint8_t s_up[RS_UP + 32];
+    __shared__ uint32_t s_qoff[T + 1], s_uoff[T + 1];
+    __shared__ uint32_t s_wsum[T / 32];
+    __shared__ unsigned long long s_prefix;
+    __shared__ __align__(8) unsigned long long s_bar[2];     // mbarriers of the two staging copies
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t tile = blockIdx.x, n = P.n, ntiles = (n + T - 1) / T;
+    if (tile < ntiles) {
+        const uint32_t q0 = tile * T, nq = min((uint32_t)T, n - q0);
+        const uint32_t barq = (uint32_t)__cvta_generic_to_shared(&s_bar[0]), baru = (uint32_t)__cvta_generic_to_shared(&s_bar[1]);
+        if (tid == 0) {
+            mbar_init(barq, 1); mbar_init(baru, 1);
+            stage_range(barq, s_q, P.q, P.q_off[q0], P.q_off[q0 + nq], RS_Q);
+            stage_range(baru, s_up, P.up, P.up_off[q0], P.up_off[q0 + nq], RS_UP);
+        }
+        if (tid < (int)nq) { s_qoff[tid] = P.q_off[q0 + tid]; s_uoff[tid] = P.up_off[q0 + tid]; }
+        if (tid == 0) { s_qoff[nq] = P.q_off[q0 + nq]; s_uoff[nq] = P.up_off[q0 + nq]; }   // a full tile has no thread 128
+        __syncthreads();
+        const uint32_t qb0 = s_qoff[0], qb1 = s_qoff[nq], ub0 = s_uoff[0], ub1 = s_uoff[nq];
+        const uint32_t qa0 = qb0 & ~15u, ua0 = ub0 & ~15u;
+        const bool q_st = stage_fits(qb0, qb1, RS_Q), u_st = stage_fits(ub0, ub1, RS_UP);
+        if (q_st && qb1 > qa0) mbar_wait(barq, 0);
+        if (u_st && ub1 > ua0) mbar_wait(baru, 0);
+
+        // ---- decode + size ----
+        Relay R;
+        R.status = ST_DROPPED; R.rlen = 0; R.keep = 0;
+        const uint8_t* qp = nullptr; const uint8_t* upp = nullptr;
+        uint32_t ul = 0;
+        if (tid < (int)nq) {
+            // a packet must lie inside its tile's byte range; an upstream that does not counts as empty (failed lookup)
+            const uint32_t o0 = s_qoff[tid], o1 = s_qoff[tid + 1], u0 = s_uoff[tid], u1 = s_uoff[tid + 1];
+            if (o0 >= qb0 && o1 >= o0 && o1 <= qb1) {
+                qp = q_st ? s_q + (o0 - qa0) : P.q + o0;
+                if (u0 >= ub0 && u1 >= u0 && u1 <= ub1) { upp = u_st ? s_up + (u0 - ua0) : P.up + u0; ul = u1 - u0; }
+                relay_size(qp, o1 - o0, upp, ul, P.tcp != 0, R);
+            }
+        }
+        // ---- CTA scan of the reply sizes (128 x 65,535 < 2^24) ----
+        const uint32_t v = R.rlen;
+        uint32_t inc = v;
+        for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
+        if (lane == 31) s_wsum[warp] = inc;
+        __syncthreads();
+        uint32_t wbase = 0, tile_bytes = 0;
+        for (int w = 0; w < T / 32; w++) { const uint32_t x = s_wsum[w]; if (w < warp) wbase += x; tile_bytes += x; }
+        const uint32_t my_o = wbase + inc - v;
+        // ---- placement ----
+        if (!ORDERED) {
+            if (tid == 0) s_prefix = atomicAdd(P.desc + P.ntiles_cap, (unsigned long long)tile_bytes);
+        } else if (warp == 0) {
+            const uint64_t ex = lookback(P.desc, tile, tile_bytes, lane);
+            if (lane == 0) s_prefix = ex;
+        }
+        __syncthreads();
+        const uint64_t gbase = s_prefix & D_VAL;
+        const bool overflow = gbase + tile_bytes > (uint64_t)P.out_cap;
+        if (tid < (int)nq) {
+            P.out_off[q0 + tid] = (uint32_t)(gbase + my_o);
+            P.out_len[q0 + tid] = (uint16_t)R.rlen;
+            P.status[q0 + tid] = (uint8_t)R.status;
+        }
+        if (overflow && tid == 0) P.totals[2] = P.epoch;
+        // ---- emit ----
+        if (!overflow) {
+            uint8_t* const dst = P.bounce ? P.bounce : P.out;
+            if (R.rlen) relay_emit(qp, upp, ul, R, dst + gbase + my_o);
+            if (P.bounce && tile_bytes) {                 // the tile's contiguous range to pinned host memory, 16 bytes per store
+                __syncthreads();
+                const uint8_t* src = P.bounce + gbase;
+                uint8_t* g = P.out + gbase;
+                uint32_t head = (uint32_t)((16 - (gbase & 15)) & 15);
+                if (head > tile_bytes) head = tile_bytes;
+                if (tid < (int)head) g[tid] = src[tid];
+                const uint32_t nv = (tile_bytes - head) >> 4;
+                for (uint32_t i = tid; i < nv; i += T) *(uint4*)(g + head + 16 * i) = *(const uint4*)(src + head + 16 * i);
+                const uint32_t x0 = head + (nv << 4);
+                for (uint32_t x = x0 + tid; x < tile_bytes; x += T) g[x] = src[x];
+            }
+        }
+    }
+    // ---- self-cleaning: the last block publishes the totals and resets the placement state ----
+    if (warp == 0) {
+        uint32_t last = 0;
+        if (lane == 0) { if (ORDERED) __threadfence(); last = atomicAdd(P.counter + 1, 1u) == gridDim.x - 1; }
+        last = __shfl_sync(0xffffffffu, last, 0);
+        if (last) {
+            __threadfence();
+            volatile unsigned long long* D = P.desc;
+            unsigned long long cur = 0;
+            if (ORDERED) { if (ntiles) cur = D[ntiles - 1] & D_VAL; }
+            else cur = D[P.ntiles_cap];
+            if (lane == 0) {
+                const uint32_t tb = (uint32_t)cur;
+                P.out_off[n] = tb; P.totals[0] = tb; P.totals[1] = 0; P.totals[3] = P.epoch;
+            }
+            __syncwarp();
+            if (ORDERED) { for (uint32_t i = lane; i < ntiles; i += 32) P.desc[i] = 0; }
+            else if (lane == 0) P.desc[P.ntiles_cap] = 0;
+            if (lane == 0) P.counter[1] = 0;
+        }
+    }
+}
 
 // ---- multi-GPU: route + push ----------------------------------------------------------------
 // Ingress side of the sharded design (SURVEY.md §8e).  Each query is parsed just far enough to
@@ -677,6 +821,10 @@ struct bb_engine {
     uint32_t* h_fb = nullptr;
     // the zone this engine last synchronised with (incremental updates only continue from that state)
     const bb_zone* zone = nullptr; uint64_t zone_gen = 0; uint64_t arena_cap = 0;
+    // bb_relay_batch's device staging: allocated on first use, grown when a batch needs more (byte capacities)
+    struct RelayBuf { void* p = nullptr; size_t cap = 0; };
+    RelayBuf r_q, r_qoff, r_up, r_upoff, r_out, r_out_off, r_out_len, r_status, r_totals;
+    const void* r_zc_seen[4] = {}; bool r_zc_ok = false;      // last output pointer set checked for being pinned
 };
 
 extern "C" {
@@ -768,6 +916,8 @@ void bb_engine_destroy(bb_engine* e) {
         if (s.ev) cudaEventDestroy(s.ev); if (s.stream) cudaStreamDestroy(s.stream);
     }
     for (int i = 0; i < e->n_dev_streams; i++) cudaFree(e->dev_desc[i]);
+    for (auto* b : { &e->r_q, &e->r_qoff, &e->r_up, &e->r_upoff, &e->r_out, &e->r_out_off, &e->r_out_len, &e->r_status, &e->r_totals })
+        cudaFree(b->p);
     cudaFree(e->d_const); cudaFree(e->d_table); cudaFree(e->d_arena);
     if (e->h_fb) cudaFreeHost(e->h_fb);
     delete e;
@@ -899,10 +1049,9 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     return BB_OK;
 }
 
-int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
-                            uint64_t seed, uint32_t qidx_base, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
-                            uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_miss_idx, uint32_t* d_totals, void* stream) {
-    if (!e || n > e->max_batch || ((uintptr_t)d_pkts & 15) || ((uintptr_t)d_out & 15)) return BB_ERR_ARG;
+// The look-back / claim scratch of device-resident launches on `stream` (one per caller stream: launches on different
+// streams may overlap; launches on one stream run in order, and every launch leaves the scratch zeroed).
+static int stream_desc(bb_engine* e, void* stream, unsigned long long** desc) {
     int si = -1;
     for (int i = 0; i < e->n_dev_streams; i++) if (e->dev_stream[i] == stream) si = i;
     if (si < 0) {
@@ -913,8 +1062,112 @@ int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t*
         CK(cudaMemset(dsc, 0, ((size_t)e->max_tiles + 4) * 8));
         si = e->n_dev_streams++; e->dev_stream[si] = stream; e->dev_desc[si] = dsc;
     }
-    return launch(e, e->dev_desc[si], d_pkts, d_pkt_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status, d_miss_idx,
+    *desc = e->dev_desc[si];
+    return BB_OK;
+}
+
+int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
+                            uint64_t seed, uint32_t qidx_base, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
+                            uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_miss_idx, uint32_t* d_totals, void* stream) {
+    if (!e || n > e->max_batch || ((uintptr_t)d_pkts & 15) || ((uintptr_t)d_out & 15)) return BB_ERR_ARG;
+    unsigned long long* desc = nullptr;
+    int rc = stream_desc(e, stream, &desc);
+    if (rc != BB_OK) return rc;
+    return launch(e, desc, d_pkts, d_pkt_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status, d_miss_idx,
                   d_totals, (cudaStream_t)stream, nullptr, 0, true);
+}
+
+// ---- recursion relay (lib/recursion.js:287-327) -------------------------------------------------------------------
+static int relay_launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_q, const uint32_t* d_q_off, const uint8_t* d_up,
+                        const uint32_t* d_up_off, uint32_t n, uint32_t flags, uint8_t* out, uint32_t out_cap, uint32_t* out_off,
+                        uint16_t* out_len, uint8_t* status, uint32_t* totals, uint8_t* bounce, cudaStream_t st) {
+    bbk::RelayParams P;
+    P.q = d_q; P.q_off = d_q_off; P.up = d_up; P.up_off = d_up_off; P.n = n;
+    P.out = out; P.out_cap = out_cap; P.out_off = out_off; P.out_len = out_len; P.status = status; P.totals = totals; P.bounce = bounce;
+    P.desc = desc; P.counter = (uint32_t*)(desc + e->max_tiles + 1); P.ntiles_cap = e->max_tiles;
+    P.epoch = (uint32_t)(++e->epoch); P.tcp = (flags & BB_BATCH_TCP) ? 1u : 0u;
+    const uint32_t ntiles = (n + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;   // an empty batch still reports its totals
+    if (e->ordered) bbk::relay_kernel<true><<<grid, bbk::T, 0, st>>>(P);
+    else bbk::relay_kernel<false><<<grid, bbk::T, 0, st>>>(P);
+    CK(cudaGetLastError());
+    e->launches++;
+    return BB_OK;
+}
+
+static int relay_grow(bb_engine::RelayBuf& b, size_t need) {
+    if (need <= b.cap) return BB_OK;
+    cudaFree(b.p); b.p = nullptr; b.cap = 0;
+    CK(cudaMalloc(&b.p, need));
+    b.cap = need;
+    return BB_OK;
+}
+
+int bb_relay_batch(bb_engine* e, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* up_pkts, const uint32_t* up_off,
+                   uint32_t n, uint32_t flags, uint8_t* out, uint32_t out_cap, uint32_t* out_off, uint16_t* out_len, uint8_t* status) {
+    if (!e || !e->hconst.recursion || !q_off || !up_off || !out_off || n > e->max_batch) return BB_ERR_ARG;
+    if (n && (!status || !out_len || !out || (q_off[n] && !q_pkts) || (up_off[n] && !up_pkts))) return BB_ERR_ARG;
+    for (uint32_t i = 0; i < n; i++) if (q_off[i + 1] < q_off[i] || up_off[i + 1] < up_off[i]) return BB_ERR_ARG;
+    const uint32_t qbytes = q_off[n], ubytes = up_off[n];
+    const bool tcp = (flags & BB_BATCH_TCP) != 0;
+    // a reply is at most 1,200 bytes over UDP and 65,535 over TCP: the device buffer never needs more than that per relay
+    const uint64_t ocap = std::min<uint64_t>(out_cap, (uint64_t)n * (tcp ? 65535u : 1200u));
+    CK(cudaSetDevice(e->device));
+    int rc;
+    if ((rc = relay_grow(e->r_q, (size_t)qbytes + 64)) || (rc = relay_grow(e->r_qoff, ((size_t)n + 1) * 4)) ||
+        (rc = relay_grow(e->r_up, (size_t)ubytes + 64)) || (rc = relay_grow(e->r_upoff, ((size_t)n + 1) * 4)) ||
+        (rc = relay_grow(e->r_out, (size_t)ocap + 64)) || (rc = relay_grow(e->r_totals, 16)))
+        return rc;
+    // zero-copy results when every output buffer is pinned host memory (bb_host_alloc), as bb_resolve_submit_ex does
+    const void* outs[4] = { out, out_off, out_len, status };
+    if (memcmp(outs, e->r_zc_seen, sizeof outs) != 0) {
+        bool ok = ((uintptr_t)out & 15) == 0;
+        for (int i = 0; ok && i < 4; i++) {
+            cudaPointerAttributes at;
+            ok = cudaPointerGetAttributes(&at, outs[i]) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer == outs[i];
+        }
+        cudaGetLastError();
+        memcpy(e->r_zc_seen, outs, sizeof outs); e->r_zc_ok = ok;
+    }
+    const bool zc = e->r_zc_ok && n != 0;
+    if (!zc && ((rc = relay_grow(e->r_out_off, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->r_out_len, (size_t)n * 2 + 16)) ||
+                (rc = relay_grow(e->r_status, (size_t)n + 16))))
+        return rc;
+    SlotCtx& s = e->slots[0];                    // the stream (and look-back state) of the synchronous resolve calls
+    if (qbytes) CK(cudaMemcpyAsync(e->r_q.p, q_pkts, qbytes, cudaMemcpyHostToDevice, s.stream));
+    if (ubytes) CK(cudaMemcpyAsync(e->r_up.p, up_pkts, ubytes, cudaMemcpyHostToDevice, s.stream));
+    CK(cudaMemcpyAsync(e->r_qoff.p, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, s.stream));
+    CK(cudaMemcpyAsync(e->r_upoff.p, up_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, s.stream));
+    uint8_t* d_out = (uint8_t*)e->r_out.p;
+    rc = zc ? relay_launch(e, s.d_desc, (uint8_t*)e->r_q.p, (uint32_t*)e->r_qoff.p, (uint8_t*)e->r_up.p, (uint32_t*)e->r_upoff.p, n, flags,
+                           out, (uint32_t)ocap, out_off, out_len, status, (uint32_t*)e->r_totals.p, d_out, s.stream)
+            : relay_launch(e, s.d_desc, (uint8_t*)e->r_q.p, (uint32_t*)e->r_qoff.p, (uint8_t*)e->r_up.p, (uint32_t*)e->r_upoff.p, n, flags,
+                           d_out, (uint32_t)ocap, (uint32_t*)e->r_out_off.p, (uint16_t*)e->r_out_len.p, (uint8_t*)e->r_status.p,
+                           (uint32_t*)e->r_totals.p, nullptr, s.stream);
+    if (rc != BB_OK) return rc;
+    const uint32_t epoch = (uint32_t)e->epoch;
+    uint32_t tot[4];
+    CK(cudaMemcpyAsync(tot, e->r_totals.p, 16, cudaMemcpyDeviceToHost, s.stream));
+    CK(cudaStreamSynchronize(s.stream));
+    if (tot[2] == epoch || tot[0] > out_cap) return BB_ERR_CAPACITY;
+    if (zc) return BB_OK;                        // everything is already in the caller's buffers
+    if (tot[0]) CK(cudaMemcpyAsync(out, d_out, tot[0], cudaMemcpyDeviceToHost, s.stream));
+    CK(cudaMemcpyAsync(out_off, e->r_out_off.p, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, s.stream));
+    if (n) CK(cudaMemcpyAsync(out_len, e->r_out_len.p, (size_t)n * 2, cudaMemcpyDeviceToHost, s.stream));
+    if (n) CK(cudaMemcpyAsync(status, e->r_status.p, n, cudaMemcpyDeviceToHost, s.stream));
+    CK(cudaStreamSynchronize(s.stream));
+    return BB_OK;
+}
+
+int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t* d_q_off, const uint8_t* d_up_pkts,
+                          const uint32_t* d_up_off, uint32_t n, uint32_t flags, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
+                          uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_totals, void* stream) {
+    if (!e || !e->hconst.recursion || n > e->max_batch || ((uintptr_t)d_q_pkts & 15) || ((uintptr_t)d_up_pkts & 15) || ((uintptr_t)d_out & 15))
+        return BB_ERR_ARG;
+    unsigned long long* desc = nullptr;
+    int rc = stream_desc(e, stream, &desc);
+    if (rc != BB_OK) return rc;
+    return relay_launch(e, desc, d_q_pkts, d_q_off, d_up_pkts, d_up_off, n, flags, d_out, out_cap, d_out_off, d_out_len, d_status,
+                        d_totals, nullptr, (cudaStream_t)stream);
 }
 
 int bb_resolve_submit_ex(bb_engine* e, int slot, const uint8_t* pkts, const uint32_t* pkt_off, uint32_t n, uint64_t seed,

@@ -155,6 +155,35 @@ class Engine(object):
                                         status.ctypes.data, miss.ctypes.data, ctypes.byref(n_miss), 1 if tcp else 0))
         return out[:out_off[n]].copy(), out_off, out_len[:n], status[:n], miss[:n_miss.value].copy()
 
+    # -- recursion relay (bb_relay_batch, lib/recursion.js:287-327) ---------------------------
+    def relay_batch(self, q_data, q_off, up_data, up_off, tcp=False, out=None):
+        """The replies to forwarded misses: query i (q_data[q_off[i]:q_off[i+1]]) answered from upstream response i
+        (up_data[up_off[i]:up_off[i+1]]; empty = the lookup failed) -> (out uint8[total], out_off uint32[n+1],
+        out_len uint16[n], status uint8[n]).  tcp: the queries arrived over TCP (no UDP size limit).  out: optional
+        (out, out_off, out_len, status) buffers to fill, e.g. pinned ones from bb_host_alloc (then returned as views)."""
+        q_data = np.ascontiguousarray(q_data, dtype=np.uint8)
+        q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
+        up_data = np.ascontiguousarray(up_data, dtype=np.uint8)
+        up_off = np.ascontiguousarray(up_off, dtype=np.uint32)
+        n = len(q_off) - 1
+        if len(up_off) != n + 1:
+            raise ValueError('q_off and up_off must have the same length')
+        if out is None:
+            out_cap = max(4096, min(n * (65535 if tcp else 1200), 0xFFFFFF00))
+            out = (np.empty(out_cap, dtype=np.uint8), np.zeros(n + 1, dtype=np.uint32), np.zeros(max(n, 1), dtype=np.uint16),
+                   np.zeros(max(n, 1), dtype=np.uint8))
+        buf, out_off, out_len, status = out
+        check(lib().bb_relay_batch(self._h, q_data.ctypes.data, q_off.ctypes.data, up_data.ctypes.data, up_off.ctypes.data, n,
+                                   1 if tcp else 0, buf.ctypes.data, len(buf), out_off.ctypes.data, out_len.ctypes.data,
+                                   status.ctypes.data))
+        return buf[:out_off[n]].copy(), out_off[:n + 1], out_len[:n], status[:n]
+
+    def relay_device(self, d_q, d_q_off, d_up, d_up_off, n, d_out, out_cap, d_out_off, d_out_len, d_status, d_totals,
+                     tcp=False, stream=0):
+        """bb_relay_batch_device; pointers are raw device addresses."""
+        check(lib().bb_relay_batch_device(self._h, d_q, d_q_off, d_up, d_up_off, n, 1 if tcp else 0, d_out, out_cap, d_out_off,
+                                          d_out_len, d_status, d_totals, stream))
+
     # -- device-buffer path (bb_resolve_batch_device); pointers are raw device addresses ------
     def resolve_device(self, d_pkts, d_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status,
                        d_miss, d_totals, stream=0):

@@ -216,6 +216,36 @@ int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t*
                             uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off, uint16_t* d_out_len, uint8_t* d_status,
                             uint32_t* d_miss_idx, uint32_t* d_totals, void* stream);
 
+/*
+ * Recursion relay: the reply binder sends for a forwarded miss, built from the upstream resolver's response.
+ * Replaces the reply construction of Recursion.prototype.resolve (lib/recursion.js:287-327): the upstream's answer RRs
+ * of type A, AAAA, TXT, PTR, CNAME and SRV with class IN are re-wrapped with owner query.name() and the upstream's TTL
+ * (names in RDATA decompressed, SRV with the upstream's priority, weight and port); other types and classes are dropped
+ * (:316-320).  A failed lookup — an empty upstream (up_off[i] == up_off[i+1]), one that is malformed, or one without
+ * answer RRs — gives REFUSED; answers that are all dropped give NOTIMP (respond() neither sets an error nor adds an
+ * answer).  Header, question echo, EDNS and truncation follow the resolve path's wire rules (DESIGN.md sections 3, 13);
+ * flags = BB_BATCH_TCP lifts the size limit to 65,535 bytes.  The upstream packets are untrusted: every read of them is
+ * bounds-checked.  Matching an upstream response to its query (ID, question) is the caller's job.
+ *
+ *   q_pkts, q_off[n+1]    the clients' query packets, packed; a query that does not decode is BB_DROPPED (no bytes)
+ *   up_pkts, up_off[n+1]  relay i's upstream response = up_pkts[up_off[i] .. up_off[i+1])
+ *   out, out_off, out_len, status   as bb_resolve_batch (status BB_ANSWERED or BB_DROPPED)
+ * Offsets must not decrease (BB_ERR_ARG).  BB_ERR_ARG also for n > max_batch and on an engine created without
+ * `recursion`; BB_ERR_CAPACITY when the replies do not fit out_cap.  When out, out_off, out_len and status are all
+ * pinned host memory (bb_host_alloc) the kernel writes the results into them directly.  Synchronous.
+ */
+int bb_relay_batch(bb_engine* e, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* up_pkts, const uint32_t* up_off,
+                   uint32_t n, uint32_t flags, uint8_t* out, uint32_t out_cap, uint32_t* out_off, uint16_t* out_len, uint8_t* status);
+/*
+ * Device-resident form of bb_relay_batch (lib/recursion.js:287-327), with the contract of bb_resolve_batch_device:
+ * d_q_pkts, d_up_pkts and d_out 16-byte aligned, the packet buffers readable up to the next multiple of 16 past their
+ * last offset; d_totals[4] = {total reply bytes, 0, overflow marker, done marker}, the markers equal to
+ * bb_engine_launch_epoch() of this call when set; up to 16 streams (shared with bb_resolve_batch_device).  Asynchronous.
+ */
+int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t* d_q_off, const uint8_t* d_up_pkts,
+                          const uint32_t* d_up_off, uint32_t n, uint32_t flags, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
+                          uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_totals, void* stream);
+
 /* Number of kernel launches bb_* calls have issued so far on this engine. */
 uint64_t bb_engine_launch_count(const bb_engine* e);
 /* Epoch (launch number, low 32 bits) of the most recent resolve call on this engine. */
