@@ -116,6 +116,106 @@ __device__ __forceinline__ void bulk_s2g(void* dst, uint32_t src, uint32_t bytes
 }
 __device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
 
+// ---- the tile pipeline of resolve_kernel and relay_kernel: stage, scan, place, flush, self-clean --------------------
+// All inline: DESIGN.md section 5 ("Code layout") measured out-of-line calls in the kernel body as a loss.
+
+// Staging: the byte range [f0, f1) of a batch goes into shared memory with one bulk copy when it fits `cap` bytes from
+// f0's 16-byte aligned start.  Thread 0 issues the copy (stage_range, after mbar_init); after a barrier every thread
+// calls stage_wait with the same range, which waits for the bytes when there are any and returns whether they were staged.
+__device__ __forceinline__ bool stage_fits(uint32_t f0, uint32_t f1, uint32_t cap) { return f1 >= f0 && f1 - (f0 & ~15u) <= cap; }
+__device__ __forceinline__ void stage_range(uint32_t bar, uint8_t* s, const uint8_t* g, uint32_t f0, uint32_t f1, uint32_t cap) {
+    const uint32_t fa = f0 & ~15u;
+    if (f1 >= f0 && f1 - fa <= cap && f1 > fa) {
+        const uint32_t bytes = (f1 - fa + 15) & ~15u;
+        mbar_expect_tx(bar, bytes);
+        bulk_g2s((uint32_t)__cvta_generic_to_shared(s), g + fa, bytes, bar);
+    }
+}
+__device__ __forceinline__ bool stage_wait(uint32_t bar, uint32_t f0, uint32_t f1, uint32_t cap) {
+    const bool staged = stage_fits(f0, f1, cap);
+    if (staged && f1 > (f0 & ~15u)) mbar_wait(bar, 0);      // the bytes have landed (and are visible to every waiting thread)
+    return staged;
+}
+
+// Exclusive CTA scan over the tile's T / 32 warps: this thread's exclusive prefix of v and the tile's total; SVC: the same
+// for a second field v2 (the service variant's copy-job counts) through s_w2.  Every thread of the block calls it.
+struct TileScan { uint32_t ex, tot, ex2, tot2; };
+template <bool SVC>
+__device__ __forceinline__ TileScan cta_scan(uint32_t v, uint32_t v2, uint32_t* s_w, uint32_t* s_w2, int lane, int warp) {
+    uint32_t inc = v, inc2 = v2;
+    for (int o = 1; o < 32; o <<= 1) {
+        uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t;
+        if (SVC) { uint32_t t2 = __shfl_up_sync(0xffffffffu, inc2, o); if (lane >= o) inc2 += t2; }
+    }
+    if (lane == 31) { s_w[warp] = inc; if (SVC) s_w2[warp] = inc2; }
+    __syncthreads();
+    uint32_t wbase = 0, tot = 0, tbase = inc2 - v2, ttot = 0;
+    for (int w = 0; w < T / 32; w++) { uint32_t x = s_w[w]; if (w < warp) wbase += x; tot += x; }
+    if (SVC) for (int w = 0; w < T / 32; w++) { uint32_t x = s_w2[w]; if (w < warp) tbase += x; ttot += x; }
+    return { wbase + inc - v, tot, tbase, ttot };
+}
+
+// Placement: where the tile's output goes -> the exclusive prefix of bytes | misses << D_MISS_SHIFT over the tiles placed
+// before it, in every thread.  !ORDERED (arrival packing): one claim per tile, an atomicAdd on the cursor at
+// desc[ntiles_cap]; it never waits.  ORDERED: the look-back (warp 0).  The result is published through s_prefix; every
+// thread of the block calls it.
+template <bool ORDERED>
+__device__ __forceinline__ uint64_t place_tile(unsigned long long* desc, uint32_t ntiles_cap, uint32_t tile, uint32_t bytes, uint32_t misses,
+                                               unsigned long long& s_prefix, int tid) {
+    const int lane = tid & 31, warp = tid >> 5;
+    if (!ORDERED) {
+        if (tid == 0) s_prefix = atomicAdd(desc + ntiles_cap, (unsigned long long)bytes | ((unsigned long long)misses << D_MISS_SHIFT));
+    } else if (warp == 0) {
+        const uint64_t ex = lookback(desc, tile, (uint64_t)bytes | ((uint64_t)misses << D_MISS_SHIFT), lane);
+        if (lane == 0) s_prefix = ex;
+    }
+    __syncthreads();
+    return s_prefix;
+}
+
+// Bytes [x0, x1) of a contiguous range to g[x0, x1) — global or pinned host memory — by every thread of the block: the
+// bytes up to 16-byte alignment, 16-byte stores, then the tail bytes (fewer than 16).  g's 16-byte phase is ga's (g's
+// offset from a 16-byte aligned base).  at(x, k) is where byte x + k is read from, with the phase of g + x + k; the
+// 16-byte stores ask for an aligned x plus k = 16 * i, so that a linear source keeps one base pointer.
+// (Every caller starts at x0 = 0; with the start folded away, ptxas spilled more in resolve_kernel<0,0,0>.)
+template <class At>
+__device__ __forceinline__ void flush_range(uint8_t* g, uint64_t ga, uint32_t x0, uint32_t x1, At at, int tid) {
+    uint32_t head = (uint32_t)((16 - ((ga + x0) & 15)) & 15);
+    if (head > x1 - x0) head = x1 - x0;
+    if (tid < (int)head) g[x0 + tid] = *at(x0 + tid, 0);
+    x0 += head;
+    const uint32_t nv = (x1 - x0) >> 4;
+    for (uint32_t i = tid; i < nv; i += T) *(uint4*)(g + x0 + 16 * i) = *(const uint4*)at(x0, 16 * i);
+    x0 += nv << 4;
+    if (x0 + tid < x1) g[x0 + tid] = *at(x0 + tid, 0);
+}
+
+// Self-cleaning, run by warp 0 of every block (blocks beyond the tiles only take part in the count): the last block to
+// finish reads the final descriptor — the inclusive prefix of the last tile, or the arrival cursor — hands it to
+// publish() in lane 0 (the kernel's totals), and resets the placement state for the next launch.
+template <bool ORDERED, class Publish>
+__device__ __forceinline__ void self_clean(unsigned long long* desc, uint32_t* counter, uint32_t ntiles, uint32_t ntiles_cap,
+                                           int lane, Publish publish) {
+    uint32_t last = 0;
+    // ORDERED: this tile's descriptor store must be visible before it counts itself done.  Arrival
+    // packing needs no fence here: the claim was an atomic whose return value this thread already
+    // consumed, so it has been performed at L2.
+    if (lane == 0) { if (ORDERED) __threadfence(); last = atomicAdd(counter + 1, 1u) == gridDim.x - 1; }
+    last = __shfl_sync(0xffffffffu, last, 0);
+    if (last) {                                    // every tile has finished reading descriptors / claiming
+        __threadfence();
+        volatile unsigned long long* D = desc;
+        unsigned long long cur = 0;
+        if (ORDERED) { if (ntiles) cur = D[ntiles - 1] & D_VAL; }            // inclusive prefix of the last tile
+        else cur = D[ntiles_cap];
+        if (lane == 0) publish(cur);
+        __syncwarp();
+        if (ORDERED) { for (uint32_t i = lane; i < ntiles; i += 32) desc[i] = 0; }
+        else if (lane == 0) desc[ntiles_cap] = 0;
+        if (lane == 0) counter[1] = 0;
+    }
+}
+
 // 6 tiles (768 threads) resident per SM: 80 registers (96 for the service variant).  On sm_90a the 64-register cap of
 // 8 tiles spills ~600 bytes per thread, and 6 measured faster on an H100 on configs 2 and 3 (DESIGN.md section 5).
 #ifndef BB_MIN_BLOCKS
@@ -182,12 +282,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     const uint32_t bar = (uint32_t)__cvta_generic_to_shared(&s_bar);
     if (tid == 0) {
         mbar_init(bar, 1);
-        const uint32_t f0 = r_pkt_off[q0], f1 = r_pkt_off[q0 + nq], fa = f0 & ~15u;
-        if (f1 >= f0 && f1 - fa <= (uint32_t)S_IN && f1 > fa) {
-            const uint32_t bytes = (f1 - fa + 15) & ~15u;
-            mbar_expect_tx(bar, bytes);
-            bulk_g2s((uint32_t)__cvta_generic_to_shared(s_in), r_pkts + fa, bytes, bar);
-        }
+        stage_range(bar, s_in, r_pkts, r_pkt_off[q0], r_pkt_off[q0 + nq], S_IN);
     }
     if (tid < (int)nq) s_off[tid] = r_pkt_off[q0 + tid];
     if (tid == 0) s_off[nq] = r_pkt_off[q0 + nq];
@@ -195,8 +290,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     STAMP(1);
     const uint32_t b0 = s_off[0], b1 = s_off[nq];
     const uint32_t a0 = b0 & ~15u;
-    const bool staged = b1 >= b0 && b1 - a0 <= S_IN;
-    if (staged && b1 > a0) mbar_wait(bar, 0);                 // the bytes have landed (and are visible to every waiting thread)
+    const bool staged = stage_wait(bar, b0, b1, S_IN);
 
     STAMP(2);
     // ---- parse + lookup + size ----------------------------------------------------------------
@@ -249,34 +343,15 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
 
     STAMP(6);
     // ---- CTA scan of (bytes, misses) ------------------------------------------------------------
-    uint32_t v = my_len | (my_miss << 24);     // 128 x 1232 < 2^24
-    uint32_t inc = v, inc2 = my_cnt;
-    for (int o = 1; o < 32; o <<= 1) {
-        uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t;
-        if (SVC) { uint32_t t2 = __shfl_up_sync(0xffffffffu, inc2, o); if (lane >= o) inc2 += t2; }
-    }
-    if (lane == 31) { s_wsum[warp] = inc; if (SVC) s_wsum2[warp] = inc2; }
-    __syncthreads();
-    uint32_t wbase = 0, tot = 0, tbase = inc2 - my_cnt, ttot = 0;
-    for (int w = 0; w < T / 32; w++) { uint32_t x = s_wsum[w]; if (w < warp) wbase += x; tot += x; }
-    if (SVC) for (int w = 0; w < T / 32; w++) { uint32_t x = s_wsum2[w]; if (w < warp) tbase += x; ttot += x; }
-    const uint32_t excl = wbase + inc - v;
-    const uint32_t my_o = excl & 0xFFFFFF, my_mrank = excl >> 24;
-    const uint32_t tile_bytes = tot & 0xFFFFFF, tile_miss = tot >> 24;
+    const TileScan sc = cta_scan<SVC>(my_len | (my_miss << 24), my_cnt, s_wsum, s_wsum2, lane, warp);     // 128 x 1232 < 2^24
+    const uint32_t my_o = sc.ex & 0xFFFFFF, my_mrank = sc.ex >> 24;
+    const uint32_t tile_bytes = sc.tot & 0xFFFFFF, tile_miss = sc.tot >> 24;
+    const uint32_t tbase = sc.ex2, ttot = sc.tot2;
 
     STAMP(7);
-    // ---- where this tile's responses (and misses) go ------------------------------------------
-    if (!ORDERED) {
-        if (tid == 0)                                    // one claim per tile: bytes | misses << 40
-            s_prefix = atomicAdd(r_desc + P.ntiles_cap, (unsigned long long)tile_bytes | ((unsigned long long)tile_miss << D_MISS_SHIFT));
-    } else
-    if (warp == 0) {
-        const uint64_t ex = lookback(r_desc, tile, (uint64_t)tile_bytes | ((uint64_t)tile_miss << D_MISS_SHIFT), lane);
-        if (lane == 0) s_prefix = ex;
-    }
-    __syncthreads();
+    // ---- where this tile's responses (and misses) go: descriptors and the claim carry bytes | misses << 40 ------------
+    const uint64_t ex = place_tile<ORDERED>(r_desc, P.ntiles_cap, tile, tile_bytes, tile_miss, s_prefix, tid);
     STAMP(8);
-    const uint64_t ex = s_prefix;
     const uint64_t gbase = ex & ((1ull << D_MISS_SHIFT) - 1);
     const uint32_t mbase = (uint32_t)(ex >> D_MISS_SHIFT);
     const bool overflow = gbase + tile_bytes > (uint64_t)P.out_cap;
@@ -321,14 +396,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
         if (r_bounce && tile_bytes) {
             __syncthreads();
             const uint8_t* src = r_bounce + gbase;
-            uint8_t* g = r_out + gbase;
-            uint32_t head = (uint32_t)((16 - (gbase & 15)) & 15);
-            if (head > tile_bytes) head = tile_bytes;
-            if (tid < (int)head) g[tid] = src[tid];
-            const uint32_t nv = (tile_bytes - head) >> 4;
-            for (uint32_t i = tid; i < nv; i += T) *(uint4*)(g + head + 16 * i) = *(const uint4*)(src + head + 16 * i);
-            const uint32_t x0 = head + (nv << 4);
-            if (x0 + tid < tile_bytes) g[x0 + tid] = src[x0 + tid];
+            flush_range(r_out + gbase, gbase, 0, tile_bytes, [=](uint32_t x, uint32_t k) { return src + x + k; }, tid);
         }
     } else if (!overflow && SVC && tile_bytes > (uint32_t)WIN) {
         const uint32_t s_out_a = (uint32_t)__cvta_generic_to_shared(s_out);
@@ -360,6 +428,8 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
             for (uint32_t j = k + 1; j < nr; j++) if (s_rstart[j] != 0xFFFFFFFFu) { x1 = s_rstart[j]; t1 = min(s_tstart[j], tv); break; }
             const uint32_t shift = (uint32_t)((gbase + x0) & 15);             // same 16-byte phase in shared and global memory
             const uint32_t delta = shift - x0;                                // tile byte x <-> s_out[delta + x]: a linear buffer
+            // The round keeps its own flush instead of flush_range (bulk copy body, head computed here): routed through the
+            // helper, resolve_kernel<0,0,1>'s spill loads grew from 92 to as much as 164 bytes per thread (-Xptxas -v).
             uint32_t head = (16u - shift) & 15u;                              // up to 16-byte alignment of the global address
             if (head > x1 - x0) head = x1 - x0;
             const uint32_t nz = (shift + (x1 - x0) + 15) >> 4;                // pieces are OR-ed into a zeroed buffer
@@ -373,11 +443,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
             // The round's bytes leave as ONE bulk copy shared -> global (16-byte aligned on both sides: the buffer keeps the
             // global address's phase), issued by one thread; the partial chunks at both ends go out as bytes.  Results
             // in pinned host memory (zero-copy, P.bounce set) keep the 16-byte stores of all threads.
-#ifdef BB_NO_BULK_FLUSH        /* experiment switch: every thread's 16-byte stores instead of the bulk copy */
-            const bool bulk = false;
-#else
             const bool bulk = r_bounce == nullptr;
-#endif
             if (bulk) fence_async_smem();                                     // this thread's writes, for the copy engine
             __syncthreads();
             if (tid < (int)head) g[x0 + tid] = s_out[delta + x0 + tid];
@@ -395,51 +461,22 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
         if (my_len) { WrT<1> w; w.begin((uint32_t)__cvta_generic_to_shared(s_out), shift + my_o); emit_fast(P, r, w, qidx); }
         __syncthreads();
         STAMP(9);
-        uint8_t* g = r_out + gbase;                                           // g[x] <-> s_out[swz(shift + x)]
-        uint32_t x0 = 0;
-        const uint32_t x1 = tile_bytes;
-        uint32_t head = (uint32_t)((16 - (gbase & 15)) & 15);                 // up to 16-byte alignment of the global address
-        if (head > x1) head = x1;
-        if (tid < (int)head) g[tid] = s_out[swz(shift + tid)];
-        x0 = head;
-        const uint32_t nv = (x1 - x0) >> 4;
-        for (uint32_t i = tid; i < nv; i += T) *(uint4*)(g + x0 + 16 * i) = *(const uint4*)(s_out + swz(shift + x0 + 16 * i));
-        x0 += nv << 4;
-        if (x0 + tid < x1) g[x0 + tid] = s_out[swz(shift + x0 + tid)];
+        flush_range(r_out + gbase, gbase, 0, tile_bytes, [=](uint32_t x, uint32_t k) { return s_out + swz(shift + x + k); }, tid);
     }
 
     STAMP(10);
     }   // tile < ntiles
-    // ---- self-cleaning: the last block to finish publishes the totals and resets the placement
-    // state for the next launch (blocks beyond ntiles only take part in this count) ------------
-    if (warp == 0) {
-        uint32_t last = 0;
-        // ORDERED: this tile's descriptor store must be visible before it counts itself done.  Arrival
-        // packing needs no fence here: the claim was an atomic whose return value this thread already
-        // consumed, so it has been performed at L2.
-        if (lane == 0) { if (ORDERED) __threadfence(); last = atomicAdd(r_counter + 1, 1u) == gridDim.x - 1; }
-        last = __shfl_sync(0xffffffffu, last, 0);
-        if (last) {                                // every tile has finished reading descriptors / claiming
-            __threadfence();
-            volatile unsigned long long* D = r_desc;
-            unsigned long long cur = 0;
-            if (ORDERED) { if (ntiles) cur = D[ntiles - 1] & D_VAL; }            // inclusive prefix of the last tile
-            else cur = D[P.ntiles_cap];
-            if (lane == 0) {
-                const uint32_t tb = (uint32_t)(cur & ((1ull << D_MISS_SHIFT) - 1));
-                r_out_off[n] = tb; r_totals[0] = tb; r_totals[1] = (uint32_t)(cur >> D_MISS_SHIFT); r_totals[3] = P.epoch;
-                // one 16-byte store (one PCIe write, no fence, nothing waits for it): what the host picks the next batch's variant from
-                if (!MULTI && P.fb) *(uint4*)P.fb = make_uint4(tb, n, 0u, P.epoch);
-                if (MULTI) {                   // what a host reading only the totals needs to know about the region
-                    r_totals[4] = n; r_totals[5] = r_n_dev ? r_n_dev[3] : 0u; r_totals[6] = P.err_in ? *(volatile const uint32_t*)P.err_in : 0u;
-                }
+    // ---- self-cleaning: the last block to finish publishes the totals and resets the placement state ----------------
+    if (warp == 0)
+        self_clean<ORDERED>(r_desc, r_counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+            const uint32_t tb = (uint32_t)(cur & ((1ull << D_MISS_SHIFT) - 1));
+            r_out_off[n] = tb; r_totals[0] = tb; r_totals[1] = (uint32_t)(cur >> D_MISS_SHIFT); r_totals[3] = P.epoch;
+            // one 16-byte store (one PCIe write, no fence, nothing waits for it): what the host picks the next batch's variant from
+            if (!MULTI && P.fb) *(uint4*)P.fb = make_uint4(tb, n, 0u, P.epoch);
+            if (MULTI) {                   // what a host reading only the totals needs to know about the region
+                r_totals[4] = n; r_totals[5] = r_n_dev ? r_n_dev[3] : 0u; r_totals[6] = P.err_in ? *(volatile const uint32_t*)P.err_in : 0u;
             }
-            __syncwarp();
-            if (ORDERED) { for (uint32_t i = lane; i < ntiles; i += 32) r_desc[i] = 0; }
-            else if (lane == 0) r_desc[P.ntiles_cap] = 0;
-            if (lane == 0) r_counter[1] = 0;
-        }
-    }
+        });
 }
 
 // ---- recursion relay (DESIGN.md section 13, lib/recursion.js:287-327) ------------------------------------------------
@@ -458,16 +495,6 @@ struct RelayParams {
     unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap;
     uint32_t epoch, tcp;
 };
-// thread 0: the byte range [f0, f1) of a batch into shared memory with one bulk copy, when it fits `cap`
-__device__ __forceinline__ bool stage_fits(uint32_t f0, uint32_t f1, uint32_t cap) { return f1 >= f0 && f1 - (f0 & ~15u) <= cap; }
-__device__ __forceinline__ void stage_range(uint32_t bar, uint8_t* s, const uint8_t* g, uint32_t f0, uint32_t f1, uint32_t cap) {
-    const uint32_t fa = f0 & ~15u;
-    if (stage_fits(f0, f1, cap) && f1 > fa) {
-        const uint32_t bytes = (f1 - fa + 15) & ~15u;
-        mbar_expect_tx(bar, bytes);
-        bulk_g2s((uint32_t)__cvta_generic_to_shared(s), g + fa, bytes, bar);
-    }
-}
 
 template <bool ORDERED>
 __global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
@@ -492,9 +519,7 @@ __global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
         __syncthreads();
         const uint32_t qb0 = s_qoff[0], qb1 = s_qoff[nq], ub0 = s_uoff[0], ub1 = s_uoff[nq];
         const uint32_t qa0 = qb0 & ~15u, ua0 = ub0 & ~15u;
-        const bool q_st = stage_fits(qb0, qb1, RS_Q), u_st = stage_fits(ub0, ub1, RS_UP);
-        if (q_st && qb1 > qa0) mbar_wait(barq, 0);
-        if (u_st && ub1 > ua0) mbar_wait(baru, 0);
+        const bool q_st = stage_wait(barq, qb0, qb1, RS_Q), u_st = stage_wait(baru, ub0, ub1, RS_UP);
 
         // ---- decode + size ----
         Relay R;
@@ -511,23 +536,10 @@ __global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
             }
         }
         // ---- CTA scan of the reply sizes (128 x 65,535 < 2^24) ----
-        const uint32_t v = R.rlen;
-        uint32_t inc = v;
-        for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(0xffffffffu, inc, o); if (lane >= o) inc += t; }
-        if (lane == 31) s_wsum[warp] = inc;
-        __syncthreads();
-        uint32_t wbase = 0, tile_bytes = 0;
-        for (int w = 0; w < T / 32; w++) { const uint32_t x = s_wsum[w]; if (w < warp) wbase += x; tile_bytes += x; }
-        const uint32_t my_o = wbase + inc - v;
+        const TileScan sc = cta_scan<false>(R.rlen, 0, s_wsum, nullptr, lane, warp);
+        const uint32_t my_o = sc.ex, tile_bytes = sc.tot;
         // ---- placement ----
-        if (!ORDERED) {
-            if (tid == 0) s_prefix = atomicAdd(P.desc + P.ntiles_cap, (unsigned long long)tile_bytes);
-        } else if (warp == 0) {
-            const uint64_t ex = lookback(P.desc, tile, tile_bytes, lane);
-            if (lane == 0) s_prefix = ex;
-        }
-        __syncthreads();
-        const uint64_t gbase = s_prefix & D_VAL;
+        const uint64_t gbase = place_tile<ORDERED>(P.desc, P.ntiles_cap, tile, tile_bytes, 0, s_prefix, tid) & D_VAL;
         const bool overflow = gbase + tile_bytes > (uint64_t)P.out_cap;
         if (tid < (int)nq) {
             P.out_off[q0 + tid] = (uint32_t)(gbase + my_o);
@@ -542,38 +554,16 @@ __global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
             if (P.bounce && tile_bytes) {                 // the tile's contiguous range to pinned host memory, 16 bytes per store
                 __syncthreads();
                 const uint8_t* src = P.bounce + gbase;
-                uint8_t* g = P.out + gbase;
-                uint32_t head = (uint32_t)((16 - (gbase & 15)) & 15);
-                if (head > tile_bytes) head = tile_bytes;
-                if (tid < (int)head) g[tid] = src[tid];
-                const uint32_t nv = (tile_bytes - head) >> 4;
-                for (uint32_t i = tid; i < nv; i += T) *(uint4*)(g + head + 16 * i) = *(const uint4*)(src + head + 16 * i);
-                const uint32_t x0 = head + (nv << 4);
-                for (uint32_t x = x0 + tid; x < tile_bytes; x += T) g[x] = src[x];
+                flush_range(P.out + gbase, gbase, 0, tile_bytes, [=](uint32_t x, uint32_t k) { return src + x + k; }, tid);
             }
         }
     }
     // ---- self-cleaning: the last block publishes the totals and resets the placement state ----
-    if (warp == 0) {
-        uint32_t last = 0;
-        if (lane == 0) { if (ORDERED) __threadfence(); last = atomicAdd(P.counter + 1, 1u) == gridDim.x - 1; }
-        last = __shfl_sync(0xffffffffu, last, 0);
-        if (last) {
-            __threadfence();
-            volatile unsigned long long* D = P.desc;
-            unsigned long long cur = 0;
-            if (ORDERED) { if (ntiles) cur = D[ntiles - 1] & D_VAL; }
-            else cur = D[P.ntiles_cap];
-            if (lane == 0) {
-                const uint32_t tb = (uint32_t)cur;
-                P.out_off[n] = tb; P.totals[0] = tb; P.totals[1] = 0; P.totals[3] = P.epoch;
-            }
-            __syncwarp();
-            if (ORDERED) { for (uint32_t i = lane; i < ntiles; i += 32) P.desc[i] = 0; }
-            else if (lane == 0) P.desc[P.ntiles_cap] = 0;
-            if (lane == 0) P.counter[1] = 0;
-        }
-    }
+    if (warp == 0)
+        self_clean<ORDERED>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+            const uint32_t tb = (uint32_t)cur;
+            P.out_off[n] = tb; P.totals[0] = tb; P.totals[1] = 0; P.totals[3] = P.epoch;
+        });
 }
 
 // ---- multi-GPU: route + push ----------------------------------------------------------------
@@ -712,17 +702,8 @@ __global__ void __launch_bounds__(T, BB_MIN_BLOCKS) route_push_kernel(const Push
             uint32_t* go = (uint32_t*)(reg + region_off_array(A.cap_q)) + gk;
             uint32_t* gq = (uint32_t*)(reg + region_qidx_array(A.cap_q)) + gk;
             for (uint32_t i = tid; i < cnt; i += T) { go[i] = s_moff[s_kstart[d] + i]; gq[i] = s_mq[s_kstart[d] + i]; }
-            uint8_t* g = reg + region_bytes(A.cap_q) + gb;                    // g[x] <-> s_sorted[s_bstart[d] + x]
             const uint8_t* sm = s_sorted + s_bstart[d];
-            uint32_t x0 = 0;
-            uint32_t head = (uint32_t)((16 - (gb & 15)) & 15);
-            if (head > nb) head = nb;
-            if (tid < (int)head) g[tid] = sm[tid];
-            x0 = head;
-            const uint32_t nv = (nb - x0) >> 4;
-            for (uint32_t i = tid; i < nv; i += T) *(uint4*)(g + x0 + 16 * i) = *(const uint4*)(sm + x0 + 16 * i);
-            x0 += nv << 4;
-            if (x0 + tid < nb) g[x0 + tid] = sm[x0 + tid];
+            flush_range(reg + region_bytes(A.cap_q) + gb, gb, 0, nb, [=](uint32_t x, uint32_t k) { return sm + x + k; }, tid);
         }
     }
     // The last block publishes the region headers (count, bytes, end-of-offsets sentinel) and then,
@@ -791,6 +772,24 @@ static thread_local std::string g_cuda_err;
 
 namespace {
 constexpr int NSLOTS = 4;
+// Whether an output set — outs[0..k), outs[0] the response bytes, which must also be 16-byte aligned — is all pinned,
+// mapped host memory (bb_host_alloc), so that a kernel can write results straight into it.  Cached for the last set
+// checked.  The answer depends on the pointers only, never on the batch: an empty batch must not cache "not pinned".
+struct PinnedCheck {
+    const void* seen[5] = {}; bool ok = false;
+    bool check(const void* const* outs, int k) {
+        if (memcmp(outs, seen, k * sizeof *outs) != 0) {
+            ok = ((uintptr_t)outs[0] & 15) == 0;
+            for (int i = 0; ok && i < k; i++) {
+                cudaPointerAttributes at;
+                ok = cudaPointerGetAttributes(&at, outs[i]) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer == outs[i];
+            }
+            cudaGetLastError();
+            memcpy(seen, outs, k * sizeof *outs);
+        }
+        return ok;
+    }
+};
 struct SlotCtx {
     cudaStream_t stream = nullptr; cudaEvent_t ev = nullptr;
     uint8_t* d_pkts = nullptr; uint32_t* d_off = nullptr; uint8_t* d_out = nullptr; uint32_t* d_out_off = nullptr;
@@ -799,7 +798,7 @@ struct SlotCtx {
     uint32_t* h_totals = nullptr;                // pinned
     // pending call
     bool busy = false, zero_copy = false; uint32_t n = 0, epoch = 0;
-    const void* zc_seen[5] = {}; bool zc_ok = false;        // last output pointer set checked for being pinned
+    PinnedCheck pinned;                          // of the caller's output sets
     uint8_t* out = nullptr; uint32_t out_cap = 0; uint32_t* miss_idx = nullptr; uint32_t* n_miss = nullptr;
 };
 }
@@ -824,8 +823,29 @@ struct bb_engine {
     // bb_relay_batch's device staging: allocated on first use, grown when a batch needs more (byte capacities)
     struct RelayBuf { void* p = nullptr; size_t cap = 0; };
     RelayBuf r_q, r_qoff, r_up, r_upoff, r_out, r_out_off, r_out_len, r_status, r_totals;
-    const void* r_zc_seen[4] = {}; bool r_zc_ok = false;      // last output pointer set checked for being pinned
+    PinnedCheck r_pinned;                        // of bb_relay_batch's output sets
 };
+
+// The zone and engine fields of the kernel parameters
+static void engine_params(const bb_engine* e, bbk::Params& P) {
+    P.table = e->d_table; P.mask = e->mask; P.arena = e->d_arena; P.ready = e->ready && e->d_table; P.eng = e->d_const;
+    P.suffix_len = e->hconst.suffix_len; P.soa_len = e->hconst.soa_len; P.recursion = e->hconst.recursion; P.lean_ok = e->hconst.lean_ok;
+}
+
+// The resolve_kernel instance for P: a multi-region launch (P.regions: a shard's receive regions, grid.y = region, small
+// variant) or one batch, in the small or the service variant; `ordered` = the engine's packing.
+static void resolve_launch(const bbk::Params& P, dim3 grid, cudaStream_t st, bool ordered, bool svc) {
+    if (P.regions) {
+        if (ordered) bbk::resolve_kernel<true, true, false><<<grid, bbk::T, 0, st>>>(P);
+        else bbk::resolve_kernel<false, true, false><<<grid, bbk::T, 0, st>>>(P);
+    } else if (svc) {
+        if (ordered) bbk::resolve_kernel<true, false, true><<<grid, bbk::T, 0, st>>>(P);
+        else bbk::resolve_kernel<false, false, true><<<grid, bbk::T, 0, st>>>(P);
+    } else {
+        if (ordered) bbk::resolve_kernel<true, false, false><<<grid, bbk::T, 0, st>>>(P);
+        else bbk::resolve_kernel<false, false, false><<<grid, bbk::T, 0, st>>>(P);
+    }
+}
 
 extern "C" {
 
@@ -1010,8 +1030,7 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     bbk::Params P;
     P.pkts = d_pkts; P.pkt_off = d_off; P.n = n; P.seed = seed; P.qidx_base = qidx_base;
     P.out = d_out; P.out_cap = out_cap; P.out_off = d_out_off; P.out_len = d_out_len; P.status = d_status; P.miss_idx = d_miss; P.totals = d_totals;
-    P.table = e->d_table; P.mask = e->mask; P.arena = e->d_arena; P.ready = e->ready && e->d_table;
-    P.eng = e->d_const; P.suffix_len = e->hconst.suffix_len; P.soa_len = e->hconst.soa_len; P.recursion = e->hconst.recursion; P.lean_ok = e->hconst.lean_ok;
+    engine_params(e, P);
     P.ntiles = (n + bbk::T - 1) / bbk::T;
     P.desc = desc; P.ntiles_cap = e->max_tiles; P.counter = (uint32_t*)(desc + e->max_tiles + 1);
     P.epoch = (uint32_t)(++e->epoch);
@@ -1037,13 +1056,7 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     const bool svc = e->profile == 2 || (e->profile == 0 && e->mean_resp >= 96);
     P.fb = (feedback && e->profile == 0) ? e->h_fb + 4 * (P.epoch % bb_engine::FB) : nullptr;
     // no memsets: the kernel leaves desc/counter zeroed for the next launch (self-cleaning)
-    if (svc) {
-        if (e->ordered) bbk::resolve_kernel<true, false, true><<<grid, bbk::T, 0, st>>>(P);
-        else bbk::resolve_kernel<false, false, true><<<grid, bbk::T, 0, st>>>(P);
-    } else {
-        if (e->ordered) bbk::resolve_kernel<true, false, false><<<grid, bbk::T, 0, st>>>(P);
-        else bbk::resolve_kernel<false, false, false><<<grid, bbk::T, 0, st>>>(P);
-    }
+    resolve_launch(P, grid, st, e->ordered, svc);
     CK(cudaGetLastError());
     e->launches++;
     return BB_OK;
@@ -1119,16 +1132,7 @@ int bb_relay_batch(bb_engine* e, const uint8_t* q_pkts, const uint32_t* q_off, c
         return rc;
     // zero-copy results when every output buffer is pinned host memory (bb_host_alloc), as bb_resolve_submit_ex does
     const void* outs[4] = { out, out_off, out_len, status };
-    if (memcmp(outs, e->r_zc_seen, sizeof outs) != 0) {
-        bool ok = ((uintptr_t)out & 15) == 0;
-        for (int i = 0; ok && i < 4; i++) {
-            cudaPointerAttributes at;
-            ok = cudaPointerGetAttributes(&at, outs[i]) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer == outs[i];
-        }
-        cudaGetLastError();
-        memcpy(e->r_zc_seen, outs, sizeof outs); e->r_zc_ok = ok;
-    }
-    const bool zc = e->r_zc_ok && n != 0;
+    const bool zc = e->r_pinned.check(outs, 4) && n != 0;
     if (!zc && ((rc = relay_grow(e->r_out_off, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->r_out_len, (size_t)n * 2 + 16)) ||
                 (rc = relay_grow(e->r_status, (size_t)n + 16))))
         return rc;
@@ -1192,33 +1196,20 @@ int bb_resolve_submit_ex(bb_engine* e, int slot, const uint8_t* pkts, const uint
     // kernel's coalesced flush writes the responses straight into it over PCIe: no device staging, no
     // D2H copies and no host round trip to learn the sizes.  Otherwise: staged copies (below).
     const void* outs[5] = { out, out_off, out_len, status, miss_idx };
-    // (whether the set is pinned does not depend on n: an empty batch must not cache "not pinned" for its buffers)
-    if (memcmp(outs, s.zc_seen, sizeof outs) != 0) {
-        bool ok = ((uintptr_t)out & 15) == 0;
-        for (int i = 0; ok && i < 5; i++) {
-            cudaPointerAttributes at;
-            ok = cudaPointerGetAttributes(&at, outs[i]) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer == outs[i];
-        }
-        cudaGetLastError();
-        memcpy(s.zc_seen, outs, sizeof outs); s.zc_ok = ok;
-    }
-    s.zero_copy = s.zc_ok && n != 0;
-    if (s.zero_copy) {
-        const uint32_t zcap = out_cap < e->out_dev_cap ? out_cap : e->out_dev_cap;    // the bounce buffer bounds it too
-        int rc = launch(e, s.d_desc, s.d_pkts, s.d_off, n, seed, qidx_base, out, zcap, out_off, out_len, status, miss_idx, s.h_totals, s.stream, s.d_out, flags);
-        if (rc != BB_OK) return rc;
-        CK(cudaEventRecord(s.ev, s.stream));
-        s.busy = true; s.n = n; s.epoch = (uint32_t)e->epoch; s.out = out; s.out_cap = out_cap; s.miss_idx = miss_idx; s.n_miss = n_miss;
-        return BB_OK;
-    }
-    uint32_t cap = out_cap < e->out_dev_cap ? out_cap : e->out_dev_cap;
-    int rc = launch(e, s.d_desc, s.d_pkts, s.d_off, n, seed, qidx_base, s.d_out, cap, s.d_out_off, s.d_out_len, s.d_status, s.d_miss, s.d_totals, s.stream, nullptr, flags);
+    const bool zc = s.zero_copy = s.pinned.check(outs, 5) && n != 0;
+    // the device staging buffer bounds the capacity either way (zero-copy tiles too large to stage assemble in it)
+    const uint32_t cap = out_cap < e->out_dev_cap ? out_cap : e->out_dev_cap;
+    int rc = launch(e, s.d_desc, s.d_pkts, s.d_off, n, seed, qidx_base, zc ? out : s.d_out, cap, zc ? out_off : s.d_out_off,
+                    zc ? out_len : s.d_out_len, zc ? status : s.d_status, zc ? miss_idx : s.d_miss, zc ? s.h_totals : s.d_totals,
+                    s.stream, zc ? s.d_out : nullptr, flags);
     if (rc != BB_OK) return rc;
-    CK(cudaMemcpyAsync(s.h_totals, s.d_totals, 16, cudaMemcpyDeviceToHost, s.stream));
+    if (!zc) CK(cudaMemcpyAsync(s.h_totals, s.d_totals, 16, cudaMemcpyDeviceToHost, s.stream));
     CK(cudaEventRecord(s.ev, s.stream));
-    CK(cudaMemcpyAsync(out_off, s.d_out_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, s.stream));
-    if (n) CK(cudaMemcpyAsync(status, s.d_status, n, cudaMemcpyDeviceToHost, s.stream));
-    if (n) CK(cudaMemcpyAsync(out_len, s.d_out_len, (size_t)n * 2, cudaMemcpyDeviceToHost, s.stream));
+    if (!zc) {
+        CK(cudaMemcpyAsync(out_off, s.d_out_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, s.stream));
+        if (n) CK(cudaMemcpyAsync(status, s.d_status, n, cudaMemcpyDeviceToHost, s.stream));
+        if (n) CK(cudaMemcpyAsync(out_len, s.d_out_len, (size_t)n * 2, cudaMemcpyDeviceToHost, s.stream));
+    }
     s.busy = true; s.n = n; s.epoch = (uint32_t)e->epoch; s.out = out; s.out_cap = out_cap; s.miss_idx = miss_idx; s.n_miss = n_miss;
     return BB_OK;
 }
@@ -1391,9 +1382,10 @@ int bb_shard_route_push(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d_pk
     for (uint32_t r = 0; r < s->nranks; r++) if (!s->x_send && !s->peer_recv[r]) return BB_ERR_ARG;
     bb_engine* e = s->e;
     bbk::PushParams A; memset(&A, 0, sizeof A);
-    A.P.pkts = d_pkts; A.P.pkt_off = d_pkt_off; A.P.n = n; A.P.eng = e->d_const; A.P.ready = 1;
-    A.P.suffix_len = e->hconst.suffix_len; A.P.soa_len = e->hconst.soa_len; A.P.recursion = e->hconst.recursion; A.P.lean_ok = e->hconst.lean_ok;
-    A.P.route = 1; A.P.nranks = s->nranks; A.P.rank = s->rank; A.P.table = e->d_table; A.P.mask = e->mask; A.P.arena = e->d_arena;
+    engine_params(e, A.P);
+    A.P.ready = 1;                                 // route mode stops at the owner rank: it never reads the zone
+    A.P.pkts = d_pkts; A.P.pkt_off = d_pkt_off; A.P.n = n;
+    A.P.route = 1; A.P.nranks = s->nranks; A.P.rank = s->rank;
     A.epoch = ++s->epoch;
     const size_t set = (size_t)(s->epoch & 1) * s->nranks;
     for (uint32_t r = 0; r < s->nranks; r++)
@@ -1433,16 +1425,13 @@ int bb_shard_resolve(bb_shard* s, uint64_t seed, int wait_for_peers, void* strea
         P.miss_idx = (uint32_t*)s->h_miss; P.totals = (uint32_t*)s->h_totals; P.qidx_out = (uint32_t*)s->h_qidx;
         P.bounce = s->d_out;                         // tiles too large to stage assemble on the device first
     }
-    P.table = e->d_table; P.mask = e->mask; P.arena = e->d_arena; P.ready = e->ready && e->d_table; P.eng = e->d_const;
-    P.suffix_len = e->hconst.suffix_len; P.soa_len = e->hconst.soa_len; P.recursion = e->hconst.recursion; P.lean_ok = e->hconst.lean_ok;
+    engine_params(e, P);
     P.ntiles = (s->cap_q + bbk::T - 1) / bbk::T; P.ntiles_cap = e->max_tiles;
     P.desc = (unsigned long long*)s->d_desc; P.counter = (uint32_t*)((unsigned long long*)s->d_desc + e->max_tiles + 1);
     P.epoch = (uint32_t)(++e->epoch); P.stage_log = nullptr; P.route = 0; P.nranks = s->nranks; P.rank = s->rank;
     P.regions = 1; P.in_stride = s->reg_size; P.out_stride = s->out_stride; P.off_stride = s->off_stride; P.len_stride = s->len_stride;
     P.status_stride = s->status_stride; P.miss_stride = s->miss_stride; P.totals_stride = s->totals_stride; P.desc_stride = s->desc_stride;
-    const dim3 grid(P.ntiles, s->nranks);
-    if (e->ordered) bbk::resolve_kernel<true, true, false><<<grid, bbk::T, 0, main>>>(P);
-    else bbk::resolve_kernel<false, true, false><<<grid, bbk::T, 0, main>>>(P);
+    resolve_launch(P, dim3(P.ntiles, s->nranks), main, e->ordered, false);
     CK(cudaGetLastError());
     s->resolve_epoch = P.epoch;
     e->launches++;

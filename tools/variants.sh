@@ -3,11 +3,10 @@
 #   tools/variants.sh build            here (no GPU): builds binder_b200/variants/lib_<name>.so for every variant
 #   tools/variants.sh run              on the GPU box: for each variant - quick parity subset, bench (value, serial,
 #                                      graph-replay launch time), 1M-batch span; the default build first and last
-# Variants: "base" (default flags), "ldg256" (-DBB_LDG256: 256-bit probe loads), "mb8" (-DBB_MIN_BLOCKS=8: 64 registers),
-# "ldg256_mb8".  Add a line to VARIANTS to try another define.
+# Variants: "base" (default flags), "mb8" (-DBB_MIN_BLOCKS=8: 64 registers).  Add a line to VARIANTS to try another define.
 set -u
 cd "$(dirname "$0")/.."
-VARIANTS=("base:" "ldg256:-DBB_LDG256" "mb8:-DBB_MIN_BLOCKS=8" "ldg256_mb8:-DBB_LDG256 -DBB_MIN_BLOCKS=8")
+VARIANTS=("base:" "mb8:-DBB_MIN_BLOCKS=8")
 FLAGS="-gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-Wno-unused-function -shared -cudart static"
 SRCS="binder_b200/csrc/engine.cu binder_b200/csrc/zone_build.cpp binder_b200/csrc/balancer_frames.cpp"
 case "${1:-}" in
