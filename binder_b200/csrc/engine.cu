@@ -582,7 +582,7 @@ struct PushParams {
     uint32_t cap_q, cap_b;                 // capacity of one region: queries, packet bytes
     unsigned long long* cursor;            // [nranks], local: count << 40 | bytes
     uint32_t* done;                        // finished-block counter
-    uint32_t* err;                         // set when a region overflows
+    uint32_t* err;                         // set when a region overflows; published in every header, then cleared
     uint32_t qidx_base, epoch;
 };
 __host__ __device__ inline size_t region_off_array(uint32_t) { return 16; }
@@ -706,9 +706,10 @@ __global__ void __launch_bounds__(T, BB_MIN_BLOCKS) route_push_kernel(const Push
             flush_range(reg + region_bytes(A.cap_q) + gb, gb, 0, nb, [=](uint32_t x, uint32_t k) { return sm + x + k; }, tid);
         }
     }
-    // The last block publishes the region headers (count, bytes, end-of-offsets sentinel) and then,
-    // with a system-scope release store, the epoch flag the owner's wait kernel acquires: the exchange
-    // needs no collective, only this ordered pair of peer stores per (source, owner).
+    // The last block publishes the region headers (count, bytes, end-of-offsets sentinel, this step's
+    // overflow flag) and then, with a system-scope release store, the epoch flag the owner's wait kernel
+    // acquires: the exchange needs no collective, only this ordered pair of peer stores per (source, owner).
+    // An overflow fails its own step only: the flag goes out in this step's headers and is then cleared.
     // A block orders its peer stores before its done count with a device-scope fence only (the barrier
     // orders every thread's stores before thread 0's fence; fences are cumulative).  The system-scope
     // release is the last block's alone: it has observed every other block's count, so by causality
@@ -720,28 +721,32 @@ __global__ void __launch_bounds__(T, BB_MIN_BLOCKS) route_push_kernel(const Push
         if (lane == 0) { __threadfence(); last = atomicAdd(A.done, 1u) == gridDim.x - 1; }
         STAMP(10);
         last = __shfl_sync(0xffffffffu, last, 0);
+        if (last) __threadfence();
+        const uint32_t ovf = last ? *(volatile uint32_t*)A.err : 0u;
         if (last && lane < (int)P.nranks) {
-            __threadfence();
             const unsigned long long c = *(volatile unsigned long long*)(A.cursor + lane);
             const uint32_t cnt = min((uint32_t)(c >> PUSH_CNT_SHIFT), A.cap_q);
             const uint32_t nb = (uint32_t)min(c & ((1ull << PUSH_CNT_SHIFT) - 1), (unsigned long long)A.cap_b);
             uint8_t* reg = A.region[lane];
             ((uint32_t*)(reg + region_off_array(A.cap_q)))[cnt] = nb;
             volatile uint32_t* hdr = (volatile uint32_t*)reg;
-            hdr[0] = cnt; hdr[1] = nb; hdr[3] = *A.err;
+            hdr[0] = cnt; hdr[1] = nb; hdr[3] = ovf;
             // the flag, released at system scope: everything above (and, by cumulativity, every other block's peer stores
             // this thread has observed through the done counter) is visible to whoever acquires it
             asm volatile("st.release.sys.global.u32 [%0], %1;" :: "l"(reg + 8), "r"(A.epoch) : "memory");
             if (P.stage_log && lane == 0) P.stage_log[(size_t)gridDim.x * NSTAGE] = gtime();   // one extra row: flag published
             A.cursor[lane] = 0;
         }
-        if (last && lane == 0) *A.done = 0;
+        __syncwarp();                                            // every lane has read the flag before it is cleared
+        if (last && lane == 0) { *A.done = 0; *A.err = 0; }
     }
 }
 
-// Owner side: wait (bounded) until every source rank has published `epoch` in its region header.
+// Owner side: wait (bounded) until every source rank has published `epoch` in its region header.  *err is this step's
+// outcome: 2 if a peer never published (timed out), else 0.
 __global__ void wait_regions_kernel(const uint8_t* recv_set, size_t reg_size, uint32_t nranks, uint32_t epoch, uint32_t* err) {
     const uint32_t r = threadIdx.x;
+    bool timed_out = false;
     if (r < nranks) {
         const uint32_t* flag = (const uint32_t*)(recv_set + (size_t)r * reg_size) + 2;
         unsigned long long spins = 0;
@@ -749,10 +754,12 @@ __global__ void wait_regions_kernel(const uint8_t* recv_set, size_t reg_size, ui
             uint32_t v;
             asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(flag) : "memory");
             if (v == epoch) break;
-            if (++spins > (1ull << 28)) { *err = 2; break; }      // ~seconds: a peer died; fail instead of hanging
+            if (++spins > (1ull << 28)) { timed_out = true; break; }      // ~seconds: a peer died; fail instead of hanging
             __nanosleep(64);
         }
     }
+    if (__any_sync(0xffffffffu, timed_out)) { if (r == 0) *err = 2; }
+    else if (r == 0) *err = 0;
 }
 
 // Incremental zone update: overwrite the listed 32-byte slots (one thread per 16-byte chunk).  Runs with no
@@ -1265,7 +1272,9 @@ struct bb_shard {
     // by the time step k+2 reuses the set, every rank has passed barrier k+1, i.e. finished resolve k.
     uint8_t* recv = nullptr;
     uint8_t* peer_recv[bbk::MAX_RANKS] = {};       // rank d's receive buffer as mapped here
-    unsigned long long* cursor = nullptr; uint32_t* done = nullptr; uint32_t* err = nullptr;
+    // done[0]: route_push's finished-block count; err (done[2]): a region of this sender's current push overflowed;
+    // werr (done[3]): the last resolve's wait for the peers timed out (2).  Each is reset by the step that uses it.
+    unsigned long long* cursor = nullptr; uint32_t* done = nullptr; uint32_t* err = nullptr; uint32_t* werr = nullptr;
     uint32_t epoch = 0;
     // owner side: one output set per source region, each kind contiguous with a fixed stride so that
     // all regions resolve in ONE launch (grid.y = region)
@@ -1310,6 +1319,7 @@ bb_shard* bb_shard_create(bb_engine* e, uint32_t nranks, uint32_t rank, uint32_t
               ck(cudaMemset(s->d_totals, 0, s->totals_stride * nranks)) &&
               ck(cudaMalloc(&s->d_desc, s->desc_stride * nranks)) && ck(cudaMemset(s->d_desc, 0, s->desc_stride * nranks));
     s->err = s->done ? s->done + 2 : nullptr;
+    s->werr = s->done ? s->done + 3 : nullptr;
     if (!ok) { bb_shard_destroy(s); return fail(BB_ERR_CUDA); }
     s->peer_recv[rank] = s->recv;
     return s;
@@ -1409,7 +1419,7 @@ int bb_shard_resolve(bb_shard* s, uint64_t seed, int wait_for_peers, void* strea
     cudaStream_t main = (cudaStream_t)stream;
     if (wait_for_peers) {
         bbk::wait_regions_kernel<<<1, 32, 0, main>>>(s->recv_base() + (size_t)(s->epoch & 1) * s->nranks * s->reg_size, s->reg_size, s->nranks,
-                                                      s->epoch, s->err);
+                                                      s->epoch, s->werr);
         CK(cudaGetLastError());
     }
     uint8_t* reg = s->recv_base() + (size_t)(s->epoch & 1) * s->nranks * s->reg_size;   // region 0 of the set just pushed
@@ -1419,7 +1429,7 @@ int bb_shard_resolve(bb_shard* s, uint64_t seed, int wait_for_peers, void* strea
     P.seed = seed; P.qidx_base = 0;
     P.out = s->d_out; P.out_cap = s->out_cap; P.out_off = (uint32_t*)s->d_out_off; P.out_len = (uint16_t*)s->d_out_len;
     P.status = s->d_status; P.miss_idx = (uint32_t*)s->d_miss; P.totals = (uint32_t*)s->d_totals;
-    P.err_in = s->err;
+    P.err_in = wait_for_peers ? s->werr : nullptr;   // totals[6]: this resolve's wait outcome (0 when it did not wait)
     if (s->host) {                                   // results straight into the pinned mirrors (zero-copy)
         P.out = s->h_out; P.out_off = (uint32_t*)s->h_out_off; P.out_len = (uint16_t*)s->h_out_len; P.status = s->h_status;
         P.miss_idx = (uint32_t*)s->h_miss; P.totals = (uint32_t*)s->h_totals; P.qidx_out = (uint32_t*)s->h_qidx;
@@ -1484,11 +1494,11 @@ int bb_shard_fetch(bb_shard* s, uint32_t src, uint8_t* out, uint32_t out_cap, ui
     if (!s || src >= s->nranks || s->host) return BB_ERR_ARG;       // host mirrors on: use bb_shard_results
     CK(cudaSetDevice(s->e->device));
     uint8_t* reg = s->recv_base() + ((size_t)(s->epoch & 1) * s->nranks + src) * s->reg_size;
-    uint32_t hdr[4], tot[4];
+    uint32_t hdr[4], tot[8];
     CK(cudaMemcpy(hdr, reg, 16, cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(tot, s->d_totals + src * s->totals_stride, 16, cudaMemcpyDeviceToHost));
-    if (hdr[3]) return BB_ERR_CAPACITY;                          // a sender overflowed this region
-    { uint32_t werr = 0; CK(cudaMemcpy(&werr, s->err, 4, cudaMemcpyDeviceToHost)); if (werr == 2) { g_cuda_err = "timed out waiting for a peer rank's push"; return BB_ERR_CUDA; } }
+    CK(cudaMemcpy(tot, s->d_totals + src * s->totals_stride, 32, cudaMemcpyDeviceToHost));
+    if (tot[6] == 2) { g_cuda_err = "timed out waiting for a peer rank's push"; return BB_ERR_CUDA; }
+    if (hdr[3]) return BB_ERR_CAPACITY;                          // the sender overflowed a region in this step
     const uint32_t n = hdr[0];
     *n_out = n; *n_miss = n ? tot[1] : 0; *total_out = n ? tot[0] : 0;
     if (!n) return BB_OK;

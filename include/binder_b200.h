@@ -286,6 +286,10 @@ void bb_engine_set_stage_log(bb_engine* e, unsigned long long* d_log);
  *   bb_shard_fetch         one region's results to host memory; qidx[] = ingress index of each
  *                          query on the source rank (qidx_base + position), which also keys the
  *                          service shuffle, so answers are identical to the unsharded engine's.
+ *                          BB_ERR_CAPACITY: the source overflowed a region (cap_q queries or cap_b =
+ *                          max_batch x bytes_per_query packet bytes) in this step, or the region's
+ *                          answers overflowed the shard's output; the step after is unaffected.
+ *                          BB_ERR_CUDA: this step's wait for the peers timed out.
  *   bb_shard_host_results  enable=1: the shard keeps pinned host mirrors of its result set and every
  *                          later bb_shard_resolve writes responses, offsets, lengths, statuses, ingress
  *                          indices, miss lists and totals straight into them (zero-copy: no device-to-

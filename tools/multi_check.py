@@ -61,6 +61,16 @@ def main():
             packed, _ = repack(reg['out'], reg['out_off'], reg['out_len'])
             want, _ = repack(o_out, o_off[:-1][local].astype(np.uint32) if len(local) else np.zeros(0, np.uint32), o_len[local])
             assert np.array_equal(packed, want), (rank, src, 'bytes')
+            # the region's miss list (region positions) names exactly the oracle's misses among its queries; the totals
+            # (query count, miss count, response bytes) agree with the arrays and with the oracle
+            miss = reg['miss'].astype(np.int64)
+            assert miss.size == 0 or miss.max() < reg['n'], (rank, src, 'miss index out of range')
+            assert np.array_equal(np.sort(local[miss]), o_miss[np.isin(o_miss, local)]), (rank, src, 'miss list')
+            assert len(miss) == int((reg['status'] == 1).sum()), (rank, src, 'miss count')
+            assert len(reg['out']) == int(reg['out_len'].astype(np.int64).sum()) == int(o_len[local].astype(np.int64).sum()), (rank, src, 'total bytes')
+            if se.engine.ordered and reg['n']:
+                assert np.array_equal(reg['out_off'][:reg['n']].astype(np.int64), np.cumsum(reg['out_len'].astype(np.int64)) - reg['out_len']), (rank, src, 'ordered offsets')
+                assert np.all(np.diff(miss) > 0), (rank, src, 'miss list not ascending')
             got[src] += reg['n']
             if src != rank:
                 nonlocal_bytes += int(reg['out_len'].sum())
