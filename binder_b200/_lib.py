@@ -49,6 +49,9 @@ SYMBOLS = {
     'bb_resolve_batch_device': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint32, _c.c_uint64,
                                            _c.c_uint32, _c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p,
                                            _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p]),
+    'bb_resolve_batch_device_ex': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint32, _c.c_uint64,
+                                              _c.c_uint32, _c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p,
+                                              _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint32]),
     'bb_relay_batch': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p,
                                                       _c.c_void_p]),
     'bb_relay_batch_device': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_uint32] + [_c.c_void_p] * 5),
@@ -62,6 +65,8 @@ SYMBOLS = {
     'bb_shard_get_ipc_handle': (_c.c_int, [_c.c_void_p, _c.c_void_p]),
     'bb_shard_open_peers': (_c.c_int, [_c.c_void_p, _c.c_void_p]),
     'bb_shard_route_push': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint32, _c.c_uint32, _c.c_void_p]),
+    'bb_shard_route_push_ex': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_uint32, _c.c_uint32, _c.c_uint32,
+                                          _c.c_void_p]),
     'bb_shard_resolve': (_c.c_int, [_c.c_void_p, _c.c_uint64, _c.c_int, _c.c_void_p]),
     'bb_shard_fetch': (_c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p, _c.c_void_p,
                                   _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p, _c.c_void_p]),

@@ -216,6 +216,10 @@ __device__ __forceinline__ void self_clean(unsigned long long* desc, uint32_t* c
     }
 }
 
+// Word 3 of a receive region's header (route_push_kernel writes it, the multi-region resolve_kernel reads it): the sender
+// overflowed a region in this step (the region is empty), and the sender pushed TCP queries (no UDP size limit).
+constexpr uint32_t HDR_OVERFLOW = 1u, HDR_TCP = 2u;
+
 // 6 tiles (768 threads) resident per SM: 80 registers (96 for the service variant).  On sm_90a the 64-register cap of
 // 8 tiles spills ~600 bytes per thread, and 6 measured faster on an H100 on configs 2 and 3 (DESIGN.md section 5).
 #ifndef BB_MIN_BLOCKS
@@ -269,8 +273,11 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     for (int i = tid; i < 64; i += T) ((uint32_t*)s_sfx)[i] = __ldg((const uint32_t*)P.eng->wire_tail + i);
     const uint32_t tile = blockIdx.x;
     STAMP(0);
-    // routed batches: size known only on the device (header: count, bytes, epoch, sender overflow flag)
-    const uint32_t n = r_n_dev ? (r_n_dev[3] ? 0u : r_n_dev[0]) : P.n;
+    // routed batches: size known only on the device (header: count, bytes, epoch, flags).  A region whose sender
+    // overflowed is empty; a region pushed over TCP is answered without the UDP size limit, whatever the other regions are.
+    const uint32_t hflags = r_n_dev ? r_n_dev[3] : 0u;
+    const uint32_t n = r_n_dev ? ((hflags & HDR_OVERFLOW) ? 0u : r_n_dev[0]) : P.n;
+    const uint32_t tcp = r_n_dev ? (hflags & HDR_TCP) : P.tcp;           // MULTI only (resolve_query<MULTI>)
     const uint32_t ntiles = (n + T - 1) / T;
     if (tile < ntiles) {
     const uint32_t q0 = tile * T;
@@ -329,7 +336,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
         if (o0 >= b0 && o1 >= o0 && o1 <= b1 && o1 - o0 <= 65535u) {
             r.p = staged ? s_in + (o0 - a0) : r_pkts + o0;
             r.sp = staged ? (uint32_t)__cvta_generic_to_shared(s_in) + (o0 - a0) : 0u;
-            resolve_query(P, r, o1 - o0, qidx, (uint32_t)__cvta_generic_to_shared(s_sfx));
+            resolve_query<MULTI>(P, r, o1 - o0, qidx, (uint32_t)__cvta_generic_to_shared(s_sfx), tcp);
         }
     }
     const uint32_t my_len = r.rlen;
@@ -582,7 +589,9 @@ struct PushParams {
     uint32_t cap_q, cap_b;                 // capacity of one region: queries, packet bytes
     unsigned long long* cursor;            // [nranks], local: count << 40 | bytes
     uint32_t* done;                        // finished-block counter
-    uint32_t* err;                         // set when a region overflows; published in every header, then cleared
+    // this step's header flags: HDR_TCP when the host set it before a TCP push (it is 0 between pushes), replaced by
+    // HDR_OVERFLOW when a region overflows (those regions are empty); published in every header, then cleared
+    uint32_t* err;
     uint32_t qidx_base, epoch;
 };
 __host__ __device__ inline size_t region_off_array(uint32_t) { return 16; }
@@ -659,7 +668,7 @@ __global__ void __launch_bounds__(T, BB_MIN_BLOCKS) route_push_kernel(const Push
             const uint32_t cnt = t >> 24, nb = t & 0xFFFFFFu;
             const uint32_t gk = (uint32_t)(base >> PUSH_CNT_SHIFT);
             const unsigned long long gb = base & ((1ull << PUSH_CNT_SHIFT) - 1);
-            if (cnt && (gk + cnt > A.cap_q || gb + nb > A.cap_b)) { s_ovf = 1; *A.err = 1; }
+            if (cnt && (gk + cnt > A.cap_q || gb + nb > A.cap_b)) { s_ovf = 1; *A.err = HDR_OVERFLOW; }
             s_kstart[d] = kk; kk += cnt;
             bb += (uint32_t)((gb - bb) & 15);      // group start has the 16-byte phase of its destination
             s_bstart[d] = bb; bb += nb;
@@ -707,9 +716,10 @@ __global__ void __launch_bounds__(T, BB_MIN_BLOCKS) route_push_kernel(const Push
         }
     }
     // The last block publishes the region headers (count, bytes, end-of-offsets sentinel, this step's
-    // overflow flag) and then, with a system-scope release store, the epoch flag the owner's wait kernel
+    // flags: overflow, TCP) and then, with a system-scope release store, the epoch flag the owner's wait kernel
     // acquires: the exchange needs no collective, only this ordered pair of peer stores per (source, owner).
-    // An overflow fails its own step only: the flag goes out in this step's headers and is then cleared.
+    // An overflow fails its own step only, and a TCP push never makes a later step TCP: the flags go out in
+    // this step's headers (every header, empty regions included) and are then cleared.
     // A block orders its peer stores before its done count with a device-scope fence only (the barrier
     // orders every thread's stores before thread 0's fence; fences are cumulative).  The system-scope
     // release is the last block's alone: it has observed every other block's count, so by causality
@@ -1086,15 +1096,22 @@ static int stream_desc(bb_engine* e, void* stream, unsigned long long** desc) {
     return BB_OK;
 }
 
-int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
-                            uint64_t seed, uint32_t qidx_base, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
-                            uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_miss_idx, uint32_t* d_totals, void* stream) {
+int bb_resolve_batch_device_ex(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
+                               uint64_t seed, uint32_t qidx_base, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
+                               uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_miss_idx, uint32_t* d_totals, void* stream,
+                               uint32_t flags) {
     if (!e || n > e->max_batch || ((uintptr_t)d_pkts & 15) || ((uintptr_t)d_out & 15)) return BB_ERR_ARG;
     unsigned long long* desc = nullptr;
     int rc = stream_desc(e, stream, &desc);
     if (rc != BB_OK) return rc;
     return launch(e, desc, d_pkts, d_pkt_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status, d_miss_idx,
-                  d_totals, (cudaStream_t)stream, nullptr, 0, true);
+                  d_totals, (cudaStream_t)stream, nullptr, flags, true);
+}
+int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
+                            uint64_t seed, uint32_t qidx_base, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
+                            uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_miss_idx, uint32_t* d_totals, void* stream) {
+    return bb_resolve_batch_device_ex(e, d_pkts, d_pkt_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status,
+                                      d_miss_idx, d_totals, stream, 0);
 }
 
 // ---- recursion relay (lib/recursion.js:287-327) -------------------------------------------------------------------
@@ -1272,7 +1289,7 @@ struct bb_shard {
     // by the time step k+2 reuses the set, every rank has passed barrier k+1, i.e. finished resolve k.
     uint8_t* recv = nullptr;
     uint8_t* peer_recv[bbk::MAX_RANKS] = {};       // rank d's receive buffer as mapped here
-    // done[0]: route_push's finished-block count; err (done[2]): a region of this sender's current push overflowed;
+    // done[0]: route_push's finished-block count; err (done[2]): the current push's header flags (TCP, or a region overflowed);
     // werr (done[3]): the last resolve's wait for the peers timed out (2).  Each is reset by the step that uses it.
     unsigned long long* cursor = nullptr; uint32_t* done = nullptr; uint32_t* err = nullptr; uint32_t* werr = nullptr;
     uint32_t epoch = 0;
@@ -1380,14 +1397,16 @@ size_t bb_shard_exchange_bytes(const bb_shard* s) { return s ? s->reg_size * s->
 uint32_t bb_shard_exchange_set(const bb_shard* s) { return s ? (s->epoch & 1) : 0; }
 // geometry of one region: [0] bytes per region, [1] capacity in queries, [2] byte offset of the u32 offset array (cap + 1
 // entries), [3] of the u32 ingress-index array (cap entries), [4] of the packed packet bytes; the first 16 bytes are the
-// header {count, packet bytes, epoch, sender overflow flag}
+// header {count, packet bytes, epoch, flags: HDR_OVERFLOW (the sender overflowed) | HDR_TCP (a TCP push)}
 void bb_shard_region_layout(const bb_shard* s, uint64_t out[5]) {
     if (!s || !out) return;
     out[0] = s->reg_size; out[1] = s->cap_q; out[2] = bbk::region_off_array(s->cap_q); out[3] = bbk::region_qidx_array(s->cap_q); out[4] = bbk::region_bytes(s->cap_q);
 }
 
-// Ingress: route every query of a device-resident batch to its owner and push it there.
-int bb_shard_route_push(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n, uint32_t qidx_base, void* stream) {
+// Ingress: route every query of a device-resident batch to its owner and push it there.  flags = BB_BATCH_TCP: the
+// queries arrived over TCP; every region header of this step says so, and the owners answer them without the UDP limit.
+int bb_shard_route_push_ex(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n, uint32_t qidx_base,
+                           uint32_t flags, void* stream) {
     if (!s || n > s->max_batch || ((uintptr_t)d_pkts & 15)) return BB_ERR_ARG;
     for (uint32_t r = 0; r < s->nranks; r++) if (!s->x_send && !s->peer_recv[r]) return BB_ERR_ARG;
     bb_engine* e = s->e;
@@ -1403,12 +1422,18 @@ int bb_shard_route_push(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d_pk
                                 : s->peer_recv[r] + (set + s->rank) * s->reg_size;    // region (this rank -> r) in r's HBM
     A.cap_q = s->cap_q; A.cap_b = s->cap_b; A.cursor = s->cursor; A.done = s->done; A.err = s->err;
     A.qidx_base = qidx_base; A.P.stage_log = e->stage_log;
+    // The flag word is 0 between pushes (this push's last block clears it): a TCP push sets its low byte to HDR_TCP, in
+    // stream order before the launch, and the last block publishes it in every header of the step.
+    if (flags & BB_BATCH_TCP) CK(cudaMemsetAsync(s->err, bbk::HDR_TCP, 1, (cudaStream_t)stream));
     // n == 0 still publishes empty region headers (one block, no queries)
     const uint32_t grid = n ? (n + bbk::T - 1) / bbk::T : 1;
     bbk::route_push_kernel<<<grid, bbk::T, 0, (cudaStream_t)stream>>>(A);
     CK(cudaGetLastError());
     e->launches++;
     return BB_OK;
+}
+int bb_shard_route_push(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n, uint32_t qidx_base, void* stream) {
+    return bb_shard_route_push_ex(s, d_pkts, d_pkt_off, n, qidx_base, 0, stream);
 }
 
 // Owner: resolve the nranks receive regions (after the caller's cross-rank barrier), one launch
@@ -1478,7 +1503,7 @@ int bb_shard_results(bb_shard* s, uint32_t src, const uint8_t** out, const uint3
     const volatile uint32_t* tot = (const volatile uint32_t*)(s->h_totals + src * s->totals_stride);
     if (tot[3] != s->resolve_epoch) return BB_ERR_ARG;
     if (tot[6] == 2) { g_cuda_err = "timed out waiting for a peer rank's push"; return BB_ERR_CUDA; }
-    if (tot[5] || tot[2] == s->resolve_epoch) return BB_ERR_CAPACITY;      // a sender overflowed the region / responses overflowed out
+    if ((tot[5] & bbk::HDR_OVERFLOW) || tot[2] == s->resolve_epoch) return BB_ERR_CAPACITY;   // a sender overflowed the region / responses overflowed out
     const uint32_t n = tot[4];
     *n_out = n; *n_miss = n ? tot[1] : 0; *total_out = n ? tot[0] : 0;
     *out = s->h_out + src * s->out_stride; *out_off = (const uint32_t*)(s->h_out_off + src * s->off_stride);
@@ -1498,7 +1523,7 @@ int bb_shard_fetch(bb_shard* s, uint32_t src, uint8_t* out, uint32_t out_cap, ui
     CK(cudaMemcpy(hdr, reg, 16, cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(tot, s->d_totals + src * s->totals_stride, 32, cudaMemcpyDeviceToHost));
     if (tot[6] == 2) { g_cuda_err = "timed out waiting for a peer rank's push"; return BB_ERR_CUDA; }
-    if (hdr[3]) return BB_ERR_CAPACITY;                          // the sender overflowed a region in this step
+    if (hdr[3] & bbk::HDR_OVERFLOW) return BB_ERR_CAPACITY;      // the sender overflowed a region in this step
     const uint32_t n = hdr[0];
     *n_out = n; *n_miss = n ? tot[1] : 0; *total_out = n ? tot[0] : 0;
     if (!n) return BB_OK;

@@ -590,7 +590,9 @@ __device__ __noinline__ uint32_t ptr_target_after_upper(uint32_t nm, uint32_t k0
 // here is exactly the name decode() accepts (and its fields are the same); anything else returns 0 and takes the
 // complete decoder and the generic path.  The lookup key is those front labels, lower-cased (zone_image.h).
 // Returns 1 when r is complete (answer sized, or DROPPED), 0 when the caller must run the general path.
-__device__ int lean_query(const Params& P, Res& r, uint32_t len, uint32_t qidx, uint32_t s_sfx) {
+// RTCP: whether the batch arrived over TCP is `tcp`, not P.tcp (resolve_query).
+template <bool RTCP>
+__device__ int lean_query(const Params& P, Res& r, uint32_t len, uint32_t qidx, uint32_t s_sfx, uint32_t tcp) {
     const uint32_t sp = r.sp;
     if (len < 12 + 2 + 5) return 0;
     const uint32_t hb = sp & ~3u, hs = (sp & 3u) * 8;
@@ -659,7 +661,7 @@ __device__ int lean_query(const Params& P, Res& r, uint32_t len, uint32_t qidx, 
     }
     // ---- a valid query (what decode() returns for it) ----
     r.qn_len = d_end + 1; r.qtype = qtype;
-    r.maxsz = P.tcp ? 65535 : r.edns ? min(max((uint32_t)r.adv, 512u), 1200u) : 512;
+    r.maxsz = (RTCP ? tcp : P.tcp) ? 65535 : r.edns ? min(max((uint32_t)r.adv, 512u), 1200u) : 512;
     const uint32_t fixed = 12 + r.qn_len + 4 + (r.edns ? 11 : 0);
     r.rk = RK_HEADER; r.rlen = fixed;
     if (r.opcode != 0 || !(qtype == QT_A || srv)) {
@@ -863,13 +865,16 @@ extern thread_local unsigned long long bb_emu_lean_count, bb_emu_general_count;
 #else
 #define BB_EMU_COUNT(x) ((void)0)
 #endif
-__device__ void resolve_query(const Params& P, Res& r, uint32_t len, uint32_t qidx, uint32_t s_sfx) {
+// RTCP (the multi-region kernel): whether the query arrived over TCP is `tcp`, the flag of its region's header, instead
+// of the launch's P.tcp.  Every other caller keeps the constant-bank flag (and the code it compiled to).
+template <bool RTCP = false>
+__device__ void resolve_query(const Params& P, Res& r, uint32_t len, uint32_t qidx, uint32_t s_sfx, uint32_t tcp = 0) {
     res_init(r);
-    if (r.sp && P.lean_ok && lean_query(P, r, len, qidx, s_sfx)) { BB_EMU_COUNT(bb_emu_lean_count); return; }
+    if (r.sp && P.lean_ok && lean_query<RTCP>(P, r, len, qidx, s_sfx, tcp)) { BB_EMU_COUNT(bb_emu_lean_count); return; }
     BB_EMU_COUNT(bb_emu_general_count);
     res_init(r);
     if (!(r.sp ? decode_staged(r.sp, len, r) : decode(r.p, len, r))) { r.status = ST_DROPPED; return; }
-    r.maxsz = P.tcp ? 65535 : r.edns ? min(max((uint32_t)r.adv, 512u), 1200u) : 512;
+    r.maxsz = (RTCP ? tcp : P.tcp) ? 65535 : r.edns ? min(max((uint32_t)r.adv, 512u), 1200u) : 512;
     const uint32_t fixed = 12 + r.qn_len + 4 + (r.edns ? 11 : 0);
     r.rk = RK_HEADER; r.rlen = fixed;
     const bool handled = r.opcode == 0 && (r.qtype == QT_A || r.qtype == QT_SRV || r.qtype == QT_PTR);

@@ -186,9 +186,10 @@ class Engine(object):
 
     # -- device-buffer path (bb_resolve_batch_device); pointers are raw device addresses ------
     def resolve_device(self, d_pkts, d_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status,
-                       d_miss, d_totals, stream=0):
-        check(lib().bb_resolve_batch_device(self._h, d_pkts, d_off, n, seed, qidx_base, d_out, out_cap,
-                                            d_out_off, d_out_len, d_status, d_miss, d_totals, stream))
+                       d_miss, d_totals, stream=0, tcp=False):
+        """bb_resolve_batch_device_ex.  tcp: the batch arrived over TCP (BB_BATCH_TCP: no UDP size limit)."""
+        check(lib().bb_resolve_batch_device_ex(self._h, d_pkts, d_off, n, seed, qidx_base, d_out, out_cap,
+                                               d_out_off, d_out_len, d_status, d_miss, d_totals, stream, 1 if tcp else 0))
 
     def close(self):
         if getattr(self, '_h', None):

@@ -125,8 +125,9 @@ class ShardedEngine(object):
             check(lib().bb_shard_host_results(h, 1 if on else 0))
         self.host_results = bool(on)
 
-    def route_push(self, d_pkts, d_off, n, qidx_base, stream, lane=0):
-        check(lib().bb_shard_route_push(self._lanes[lane], d_pkts, d_off, n, qidx_base, stream))
+    def route_push(self, d_pkts, d_off, n, qidx_base, stream, lane=0, tcp=False):
+        """bb_shard_route_push_ex.  tcp: the batch arrived over TCP; its owners answer it without the UDP size limit."""
+        check(lib().bb_shard_route_push_ex(self._lanes[lane], d_pkts, d_off, n, qidx_base, 1 if tcp else 0, stream))
 
     def barrier(self):
         """sync='nccl': cross-rank barrier in stream order (1-element all-reduce)."""
@@ -180,8 +181,8 @@ class ShardedEngine(object):
             for w in dist.batch_isend_irecv(ops):
                 w.wait()
 
-    def step(self, d_pkts, d_off, n, qidx_base, seed, stream, lane=0):
-        self.route_push(d_pkts, d_off, n, qidx_base, stream, lane)
+    def step(self, d_pkts, d_off, n, qidx_base, seed, stream, lane=0, tcp=False):
+        self.route_push(d_pkts, d_off, n, qidx_base, stream, lane, tcp)
         if self.sync == 'nccl':
             self.barrier()
         elif self.sync == 'nccl_a2a':

@@ -215,6 +215,15 @@ int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t*
                             uint64_t shuffle_seed, uint32_t qidx_base,
                             uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off, uint16_t* d_out_len, uint8_t* d_status,
                             uint32_t* d_miss_idx, uint32_t* d_totals, void* stream);
+/*
+ * bb_resolve_batch_device for batches that arrived over TCP: flags = BB_BATCH_TCP lifts the 512-byte / EDNS size limit
+ * exactly as in bb_resolve_batch_ex (a response up to 65,535 bytes, TC only beyond that; out_cap must allow for the larger
+ * answers, else the overflow marker is set).  Other bits are ignored; flags = 0 is bb_resolve_batch_device.
+ */
+int bb_resolve_batch_device_ex(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
+                               uint64_t shuffle_seed, uint32_t qidx_base,
+                               uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off, uint16_t* d_out_len, uint8_t* d_status,
+                               uint32_t* d_miss_idx, uint32_t* d_totals, void* stream, uint32_t flags);
 
 /*
  * Recursion relay: the reply binder sends for a forwarded miss, built from the upstream resolver's response.
@@ -308,6 +317,16 @@ int bb_shard_get_ipc_handle(bb_shard* s, void* handle_out);
 int bb_shard_open_peers(bb_shard* s, const void* handles);
 int bb_shard_route_push(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
                         uint32_t qidx_base, void* stream);
+/*
+ * bb_shard_route_push for a batch of TCP queries: flags = BB_BATCH_TCP makes every query of this push a TCP query.  The
+ * flag travels in each region header of the step, so each owner answers each region under its own source's limit: one
+ * step may mix ranks that push TCP with ranks that push UDP, and every push rewrites the flag.  TCP answers share the
+ * region's output room, out_cap = cap_q x 256 bytes (cap_q = max_batch): a region whose answers do not fit is
+ * BB_ERR_CAPACITY from bb_shard_fetch / bb_shard_results for that step only.  Other bits are ignored; flags = 0 is
+ * bb_shard_route_push.
+ */
+int bb_shard_route_push_ex(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
+                           uint32_t qidx_base, uint32_t flags, void* stream);
 int bb_shard_resolve(bb_shard* s, uint64_t shuffle_seed, int wait_for_peers, void* stream);
 int bb_shard_fetch(bb_shard* s, uint32_t src, uint8_t* out, uint32_t out_cap, uint32_t* out_off,
                    uint16_t* out_len, uint8_t* status, uint32_t* qidx, uint32_t* miss_idx,
@@ -321,7 +340,8 @@ int bb_shard_fetch(bb_shard* s, uint32_t src, uint8_t* out, uint32_t out_cap, ui
  *   bb_shard_exchange_set     set (0/1) the last route_push wrote = the one the next resolve reads
  *   bb_shard_region_layout    out[5] = {bytes per region, capacity in queries, offset of the u32 offsets array (cap+1), of the
  *                             u32 ingress-index array (cap), of the packet bytes}; a region starts with the 16-byte header
- *                             {count, packet bytes, epoch, sender overflow flag} */
+ *                             {count, packet bytes, epoch, flags}; flags bit 0 = the sender overflowed a region in this
+ *                             step, bit 1 = the push was TCP (bb_shard_route_push_ex) */
 int      bb_shard_use_exchange_buffers(bb_shard* s, void* d_send, void* d_recv);
 size_t   bb_shard_exchange_bytes(const bb_shard* s);
 uint32_t bb_shard_exchange_set(const bb_shard* s);

@@ -1,6 +1,8 @@
 """Sharded multi-GPU parity check (run under torchrun, one rank per GPU):
 every query of every rank's ingress batch must be answered exactly once, by the rank that owns
-its key, with the bytes the single-engine CPU oracle produces for (seed, ingress index)."""
+its key, with the bytes the single-engine CPU oracle produces for (seed, ingress index).
+--tcp: every rank pushes its batches as TCP queries (bb_shard_route_push_ex, BB_BATCH_TCP), checked against the oracle's
+TCP answers (no UDP size limit)."""
 import os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [ROOT, os.path.join(ROOT, 'oracle')]
@@ -19,6 +21,7 @@ def main():
     if rank == 0:
         build.build()
     dist.barrier()
+    tcp = '--tcp' in sys.argv[1:]
     B = int(os.environ.get('BB_BATCH', '20000'))
     zone = synth.gen_zone(int(os.environ.get('BB_ZONE', '200000')), service_frac=0.15)
     se = ShardedEngine(zone.dns_domain, zone.datacenter, zone.jsonl, rank, world, lr, max_batch=B, recursion=True,
@@ -38,14 +41,14 @@ def main():
         n = len(off) - 1
         d_pk = torch.from_numpy(data).to(dev); d_off = torch.from_numpy(off.view(np.int32)).to(dev)
         seed = 0xB1DDE5 + rnd
-        se.step(d_pk.data_ptr(), d_off.data_ptr(), n, rank * B, seed, st.cuda_stream)
+        se.step(d_pk.data_ptr(), d_off.data_ptr(), n, rank * B, seed, st.cuda_stream, tcp=tcp)
         torch.cuda.synchronize()
         got = torch.zeros(world, dtype=torch.int64, device=dev)
         nonlocal_bytes = 0
         for src in range(world):
             reg = se.fetch(src)
             sdata, soff = ingress(src, rnd)
-            o_out, o_off, o_len, o_st, o_miss = orc.resolve_batch(sdata, soff, seed=seed, qidx_base=src * B)
+            o_out, o_off, o_len, o_st, o_miss = orc.resolve_batch(sdata, soff, seed=seed, qidx_base=src * B, tcp=tcp)
             local = reg['qidx'].astype(np.int64) - src * B
             assert local.min(initial=0) >= 0 and local.max(initial=0) < len(soff) - 1
             assert len(np.unique(local)) == len(local), 'a query was delivered twice'
@@ -80,7 +83,7 @@ def main():
             print('round %d ok: %s queries/rank routed over %d ranks (rank 0 owned %d from peers)' % (rnd, B, world, int(se.fetch(1 % world)['n'])), flush=True)
     dist.barrier()
     if rank == 0:
-        print('MULTI_CHECK_OK world=%d' % world, flush=True)
+        print('MULTI_CHECK_OK world=%d%s' % (world, ' tcp' if tcp else ''), flush=True)
     dist.destroy_process_group()
 
 
