@@ -228,6 +228,32 @@ extern "C" void bb_emu_path_counts(unsigned long long* out, int reset) {
     if (reset) bbk::bb_emu_lean_count = bbk::bb_emu_general_count = 0;
 }
 
+// Where a key lives in a built zone's table (tests/test_table_probe.py proves the states it crafts with this): the table
+// mask, both hashes, the slot that holds the key (UINT32_MAX: neither of its two slots does) and whether the key's FIRST
+// position carries SLOT_DISPLACED.  `key` is the canonical form (forward: wire labels; reverse: the address string).  The
+// bytes are compared here, on the image itself, not through the builder's lookup.  Returns 1 when the key is present.
+extern "C" int bb_emu_slot_of(const bb_zone* zone, uint32_t ns, const uint8_t* key, uint32_t len, uint32_t* mask, uint32_t* slot,
+                              int* first_displaced, uint32_t* h_out, uint32_t* h2_out) {
+    const bb::ZoneImage* img = zone ? bb_zone_image(zone) : nullptr;
+    if (!img || !img->slots) return -1;
+    uint32_t h2;
+    const uint32_t h = bb::hash_key2(ns, key, len, &h2), m = img->nslots - 1;
+    *mask = m; *h_out = h; *h2_out = h2; *slot = 0xFFFFFFFFu;
+    *first_displaced = (img->slots[bb::slot1_of(h, m)].flags & bb::SLOT_DISPLACED) ? 1 : 0;
+    for (uint32_t i : { bb::slot1_of(h, m), bb::slot2_of(h, h2, m) }) {
+        const bb::Slot& s = img->slots[i];
+        if (s.kind == bb::K_EMPTY || s.ns != ns) continue;
+        const uint8_t* kb = nullptr;
+        if (s.klen == bb::KLEN_OVERFLOW) {
+            uint32_t off, l;
+            memcpy(&off, s.key, 4); memcpy(&l, s.key + 4, 4);
+            if (l == len && off + (uint64_t)len <= img->arena_len) kb = img->arena + off;
+        } else if (s.klen == len) kb = s.key;
+        if (kb && memcmp(kb, key, len) == 0) { *slot = i; return 1; }
+    }
+    return 0;
+}
+
 // Route mode (the ingress half of the sharded path, route_push_kernel's per-query step): which rank owns each
 // query's lookup key; queries that need no lookup stay on `rank`.
 extern "C" int bb_emu_route_batch(const char* dns_domain, int recursion, const uint8_t* pkts, const uint32_t* pkt_off, uint32_t n,
