@@ -182,6 +182,139 @@ static napi_value RelayBatch(napi_env env, napi_callback_info info) {
     return res;
 }
 
+// ---- TCP proxy sessions from mname-balancer (bb_tcp_hub): route a new AF_UNIX connection whose first frame is
+// INBOUND_TCP here.  Session ids travel as Uint32Array(1), counters as BigUint64Array.
+//   tcpHubCreate(engine, maxBatch) -> hub          tcpHubOpen(hub) -> Uint32Array [session]
+//   tcpHubFeed(hub, session, Buffer)  (throws on a protocol error: the session reads nothing more; drain it, then close)
+//   tcpHubEof(hub, session)          tcpHubFlush(hub, seed: BigInt) -> misses {pkts: Buffer, pktOff: Uint32Array, session: Uint32Array}
+//   tcpHubOutput(hub, session) -> {out: Buffer, closable: Uint8Array(1)}     tcpHubConsume(hub, session, nBytes)
+//   tcpHubClose(hub, session)        tcpHubRelay(hub, pkts, pktOff, upstream, upOff, sessions: Uint32Array)
+//   tcpHubStats(hub) -> BigUint64Array(11)   (bb_tcp_hub_stat 0..10)
+static napi_value U32Array(napi_env env, const uint32_t* src, size_t n) {
+    void* p; napi_value ab, t;
+    if (napi_create_arraybuffer(env, n * 4, &p, &ab) != napi_ok || napi_create_typedarray(env, napi_uint32_array, n, ab, 0, &t) != napi_ok) return nullptr;
+    if (n) memcpy(p, src, n * 4);
+    return t;
+}
+static napi_value CopyBuffer(napi_env env, const uint8_t* src, size_t n) {
+    void* p; napi_value b;
+    if (napi_create_buffer(env, n, &p, &b) != napi_ok) return nullptr;
+    if (n) memcpy(p, src, n);
+    return b;
+}
+static napi_value TcpHubCreate(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* e; NAPI_OK(napi_get_value_external(env, argv[0], &e));
+    uint32_t maxb = 4096; if (argc > 1) napi_get_value_uint32(env, argv[1], &maxb);
+    int err = 0;
+    bb_tcp_hub* h = bb_tcp_hub_create((bb_engine*)e, maxb, &err);
+    if (!h) return Throw(env, err);
+    napi_value ext;
+    NAPI_OK(napi_create_external(env, h, [](napi_env, void* p, void*) { bb_tcp_hub_destroy((bb_tcp_hub*)p); }, nullptr, &ext));
+    return ext;
+}
+static napi_value TcpHubOpen(napi_env env, napi_callback_info info) {
+    size_t argc = 1; napi_value argv[1];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; NAPI_OK(napi_get_value_external(env, argv[0], &h));
+    uint32_t sid = 0; int rc = bb_tcp_hub_open((bb_tcp_hub*)h, &sid);
+    if (rc != BB_OK) return Throw(env, rc);
+    return U32Array(env, &sid, 1);
+}
+// hub and session of a tcpHub* call (argv[0], argv[1])
+static bool HubSession(napi_env env, napi_value* argv, void** h, uint32_t* sid) {
+    return napi_get_value_external(env, argv[0], h) == napi_ok && napi_get_value_uint32(env, argv[1], sid) == napi_ok;
+}
+static napi_value TcpHubFeed(napi_env env, napi_callback_info info) {
+    size_t argc = 3; napi_value argv[3];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; uint32_t sid; if (!HubSession(env, argv, &h, &sid)) return Throw(env, BB_ERR_ARG);
+    void* data; size_t len; NAPI_OK(napi_get_buffer_info(env, argv[2], &data, &len));
+    int rc = bb_tcp_hub_feed((bb_tcp_hub*)h, sid, (const uint8_t*)data, len);
+    if (rc != BB_OK) return Throw(env, rc);
+    return nullptr;
+}
+static napi_value TcpHubEof(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; uint32_t sid; if (!HubSession(env, argv, &h, &sid)) return Throw(env, BB_ERR_ARG);
+    int rc = bb_tcp_hub_eof((bb_tcp_hub*)h, sid);
+    if (rc != BB_OK) return Throw(env, rc);
+    return nullptr;
+}
+static napi_value TcpHubFlush(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; NAPI_OK(napi_get_value_external(env, argv[0], &h));
+    uint64_t seed = 0; bool lossless; napi_get_value_bigint_uint64(env, argv[1], &seed, &lossless);
+    bb_tcp_hub_misses m; memset(&m, 0, sizeof m);
+    int rc = bb_tcp_hub_flush((bb_tcp_hub*)h, seed, &m);
+    if (rc == BB_ERR_ARG) return Throw(env, rc);              // a failed batch is counted (tcpHubStats), not thrown
+    napi_value res; NAPI_OK(napi_create_object(env, &res));
+    const uint32_t zero = 0;
+    napi_set_named_property(env, res, "pkts", CopyBuffer(env, m.pkts, m.n ? m.pkt_off[m.n] : 0));
+    napi_set_named_property(env, res, "pktOff", U32Array(env, m.n ? m.pkt_off : &zero, (size_t)m.n + 1));
+    napi_set_named_property(env, res, "session", U32Array(env, m.session, m.n));
+    return res;
+}
+static napi_value TcpHubOutput(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; uint32_t sid; if (!HubSession(env, argv, &h, &sid)) return Throw(env, BB_ERR_ARG);
+    const uint8_t* out; size_t len; int closable = 0;
+    int rc = bb_tcp_hub_output((bb_tcp_hub*)h, sid, &out, &len, &closable);
+    if (rc != BB_OK) return Throw(env, rc);
+    void* cp; napi_value ab, cl, res;
+    NAPI_OK(napi_create_arraybuffer(env, 1, &cp, &ab)); NAPI_OK(napi_create_typedarray(env, napi_uint8_array, 1, ab, 0, &cl));
+    *(uint8_t*)cp = (uint8_t)closable;
+    NAPI_OK(napi_create_object(env, &res));
+    napi_set_named_property(env, res, "out", CopyBuffer(env, out, len));
+    napi_set_named_property(env, res, "closable", cl);
+    return res;
+}
+static napi_value TcpHubConsume(napi_env env, napi_callback_info info) {
+    size_t argc = 3; napi_value argv[3];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; uint32_t sid, n; if (!HubSession(env, argv, &h, &sid)) return Throw(env, BB_ERR_ARG);
+    NAPI_OK(napi_get_value_uint32(env, argv[2], &n));
+    int rc = bb_tcp_hub_consume((bb_tcp_hub*)h, sid, n);
+    if (rc != BB_OK) return Throw(env, rc);
+    return nullptr;
+}
+static napi_value TcpHubClose(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; uint32_t sid; if (!HubSession(env, argv, &h, &sid)) return Throw(env, BB_ERR_ARG);
+    int rc = bb_tcp_hub_close((bb_tcp_hub*)h, sid);
+    if (rc != BB_OK) return Throw(env, rc);
+    return nullptr;
+}
+static napi_value TcpHubRelay(napi_env env, napi_callback_info info) {
+    size_t argc = 6; napi_value argv[6];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; NAPI_OK(napi_get_value_external(env, argv[0], &h));
+    void* pk; size_t pklen; NAPI_OK(napi_get_buffer_info(env, argv[1], &pk, &pklen));
+    void* up; size_t uplen; NAPI_OK(napi_get_buffer_info(env, argv[3], &up, &uplen));
+    const uint32_t *qo, *uo; size_t qn, un;
+    if (!check_off(env, argv[2], pklen, &qo, &qn) || !check_off(env, argv[4], uplen, &uo, &un) || qn != un) return Throw(env, BB_ERR_ARG);
+    napi_typedarray_type tt; size_t sn; void* sp; napi_value ab; size_t bo;
+    if (napi_get_typedarray_info(env, argv[5], &tt, &sn, &sp, &ab, &bo) != napi_ok || tt != napi_uint32_array || sn != qn - 1)
+        return Throw(env, BB_ERR_ARG);
+    int rc = bb_tcp_hub_relay((bb_tcp_hub*)h, (const uint8_t*)pk, qo, (const uint8_t*)up, uo, (const uint32_t*)sp, (uint32_t)sn);
+    if (rc == BB_ERR_ARG) return Throw(env, rc);              // a failed batch is counted, not thrown
+    return nullptr;
+}
+static napi_value TcpHubStats(napi_env env, napi_callback_info info) {
+    size_t argc = 1; napi_value argv[1];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; NAPI_OK(napi_get_value_external(env, argv[0], &h));
+    void* p; napi_value ab, t;
+    NAPI_OK(napi_create_arraybuffer(env, 11 * 8, &p, &ab)); NAPI_OK(napi_create_typedarray(env, napi_biguint64_array, 11, ab, 0, &t));
+    for (int i = 0; i < 11; i++) ((uint64_t*)p)[i] = bb_tcp_hub_stat((const bb_tcp_hub*)h, i);
+    return t;
+}
+
 static napi_value Init(napi_env env, napi_value exports) {
     napi_property_descriptor d[] = {
         { "zoneBuild", nullptr, ZoneBuild, nullptr, nullptr, nullptr, napi_default, nullptr },
@@ -192,6 +325,16 @@ static napi_value Init(napi_env env, napi_value exports) {
         { "engineSetRecursionFilter", nullptr, EngineSetRecursionFilter, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "resolveBatch", nullptr, ResolveBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "relayBatch", nullptr, RelayBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubCreate", nullptr, TcpHubCreate, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubOpen", nullptr, TcpHubOpen, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubFeed", nullptr, TcpHubFeed, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubEof", nullptr, TcpHubEof, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubFlush", nullptr, TcpHubFlush, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubOutput", nullptr, TcpHubOutput, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubConsume", nullptr, TcpHubConsume, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubClose", nullptr, TcpHubClose, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubRelay", nullptr, TcpHubRelay, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubStats", nullptr, TcpHubStats, nullptr, nullptr, nullptr, napi_default, nullptr },
     };
     napi_define_properties(env, exports, sizeof d / sizeof d[0], d);
     return exports;

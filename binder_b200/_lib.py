@@ -80,6 +80,18 @@ SYMBOLS = {
     'bb_backend_destroy': (None, [_c.c_void_p]),
     'bb_backend_feed': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_uint64, _c.c_void_p, _c.c_void_p, _c.c_void_p]),
     'bb_backend_stat': (_c.c_uint64, [_c.c_void_p, _c.c_int]),
+    'bb_tcp_hub_create': (_c.c_void_p, [_c.c_void_p, _c.c_uint32, _c.POINTER(_c.c_int)]),
+    'bb_tcp_hub_destroy': (None, [_c.c_void_p]),
+    'bb_tcp_hub_open': (_c.c_int, [_c.c_void_p, _c.c_void_p]),
+    'bb_tcp_hub_feed': (_c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_size_t]),
+    'bb_tcp_hub_eof': (_c.c_int, [_c.c_void_p, _c.c_uint32]),
+    'bb_tcp_hub_flush': (_c.c_int, [_c.c_void_p, _c.c_uint64, _c.c_void_p]),
+    'bb_tcp_hub_output': (_c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p, _c.c_void_p]),
+    'bb_tcp_hub_consume': (_c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_size_t]),
+    'bb_tcp_hub_close': (_c.c_int, [_c.c_void_p, _c.c_uint32]),
+    'bb_tcp_hub_relay': (_c.c_int, [_c.c_void_p] * 6 + [_c.c_uint32]),
+    'bb_tcp_hub_peer': (_c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p]),
+    'bb_tcp_hub_stat': (_c.c_uint64, [_c.c_void_p, _c.c_int]),
     'bb_host_alloc': (_c.c_void_p, [_c.c_size_t]),
     'bb_host_free': (None, [_c.c_void_p]),
 }

@@ -12,8 +12,18 @@ Frames are already "batched raw packets + source address", i.e. exactly the engi
 container plus 12 bytes of addressing per packet.  This module turns a buffer of frames into a
 batch for bb_resolve_batch and the results back into OUTBOUND_UDP frames; HELLO / HEARTBEAT frames
 are answered in place.  numpy only: no per-packet Python on the hot path.
+
+DNS-over-TCP clients reach a backend differently: the balancer hands each client connection over as its own AF_UNIX
+session that opens with INBOUND_TCP {3, source IPv4, source port} (12 bytes), is answered INBOUND_TCP_OK (1003) and
+then carries the client's raw 2-byte length-prefixed DNS stream both ways (backend.c:60-75, tcp_proxy.c:160-300).
+TcpHub / NativeTcpHub hold many such sessions and resolve the messages that complete on all of them as one TCP batch.
+A host routes a new AF_UNIX connection by its first frame: CLIENT_HELLO to a Backend, INBOUND_TCP to the hub.
 """
+import struct
+
 import numpy as np
+
+from .server import TcpFramer, pack_packets
 
 CLIENT_HELLO, INBOUND_UDP, INBOUND_TCP, CLIENT_HEARTBEAT = 1, 2, 3, 4
 SERVER_HELLO, OUTBOUND_UDP, INBOUND_TCP_OK, SERVER_HEARTBEAT = 1001, 1002, 1003, 1004
@@ -186,5 +196,276 @@ class NativeBackend(object):
     def __del__(self):
         try:
             self.close()
+        except Exception:
+            pass
+
+
+# ---- TCP proxy sessions: many sessions, one batch per flush ---------------------------------------------
+HUB_STATS = ('sessions', 'messages', 'answered', 'missed', 'dropped', 'protocol_errors', 'failed', 'relayed', 'open', 'queued')
+
+
+class _TcpSession(object):
+    __slots__ = ('pre', 'framer', 'shook', 'eof', 'bad', 'queued', 'relays', 'out', 'ip', 'port')
+
+    def __init__(self):
+        self.pre, self.framer, self.out = b'', TcpFramer(), bytearray()
+        self.shook = self.eof = self.bad = False
+        self.queued = self.relays = self.ip = self.port = 0
+
+
+class TcpHub(object):
+    """The TCP hub (bb_tcp_hub, include/binder_b200.h) in Python, around an injected resolver (Engine or the CPU oracle)
+    and relayer (anything with relay_batch(q_data, q_off, up_data, up_off, tcp=True); the resolver by default).
+
+    open() -> session id; feed(id, bytes) -> False on a protocol error; eof(id); flush(seed) -> [(miss packet, id)];
+    output(id) -> (bytes to write, closable); consume(id, n); close(id); relay(queries, upstreams, ids).  Limits as the
+    native hub's: max_batch queries and max_batch_bytes query bytes per batch, out_cap answer bytes per batch (None: the
+    resolver's own limit).  A batch the resolver fails, or whose answers exceed out_cap, loses its queries (counted)."""
+
+    def __init__(self, resolver, max_batch=4096, max_batch_bytes=None, out_cap=None, relayer=None):
+        self.resolver, self.relayer = resolver, relayer if relayer is not None else resolver
+        self.max_batch = max_batch
+        self.max_bytes = max_batch_bytes if max_batch_bytes is not None else max(64 * max_batch, 1 << 16)
+        self.out_cap = out_cap
+        self.sessions, self.next_id, self.queue = {}, 1, []
+        self.counters = dict.fromkeys(HUB_STATS[:8], 0)
+
+    def _get(self, sid):
+        s = self.sessions.get(sid)
+        if s is None:
+            raise KeyError('no open session %r' % (sid,))
+        return s
+
+    def open(self):
+        sid, self.next_id = self.next_id, self.next_id + 1
+        self.sessions[sid] = _TcpSession()
+        self.counters['sessions'] += 1
+        return sid
+
+    def feed(self, sid, chunk):
+        s, c = self._get(sid), self.counters
+        if s.eof:
+            raise KeyError('session %r is past eof' % (sid,))
+        if s.bad:
+            return False
+        chunk = bytes(chunk)
+        if not s.shook:
+            s.pre += chunk
+            if len(s.pre) < 4:
+                return True
+            if struct.unpack_from('<I', s.pre)[0] != INBOUND_TCP:     # CLIENT_HELLO, INBOUND_UDP, ...: not a TCP session
+                s.bad, s.pre = True, b''
+                c['protocol_errors'] += 1
+                return False
+            if len(s.pre) < 12:
+                return True
+            _, s.ip, s.port = struct.unpack_from('<III', s.pre)
+            s.shook, s.out = True, s.out + struct.pack('<I', INBOUND_TCP_OK)
+            chunk, s.pre = s.pre[12:], b''
+        msgs = s.framer.feed(chunk)
+        self.queue += [(m, sid) for m in msgs]
+        s.queued += len(msgs)
+        c['messages'] += len(msgs)
+        if s.framer.bad:                             # zero-length message: what completed before it is still answered
+            s.bad = True
+            s.framer.buf.clear()
+            c['protocol_errors'] += 1
+            return False
+        return True
+
+    def eof(self, sid):
+        s = self._get(sid)
+        s.eof, s.pre = True, b''
+        s.framer.buf.clear()
+
+    def _answers(self, fn, *args):
+        """resolve/relay one batch -> results, or None when it failed"""
+        try:
+            res = fn(*args, tcp=True)
+        except Exception:                            # BinderError (capacity, CUDA), as Server._resolve
+            return None
+        if self.out_cap is not None and int(np.asarray(res[2], dtype=np.int64).sum()) > self.out_cap:
+            return None
+        return res
+
+    def flush(self, seed):
+        queue, self.queue, c = self.queue, [], self.counters
+        misses, qidx, i = [], 0, 0
+        while i < len(queue):
+            batch, nbytes = [], 0
+            while i < len(queue) and len(batch) < self.max_batch:
+                m, sid = queue[i]
+                s = self.sessions.get(sid)
+                if s is None or len(m) > self.max_bytes:
+                    c['dropped'] += 1
+                    if s is not None:
+                        s.queued -= 1
+                    i += 1
+                    continue
+                if nbytes + len(m) > self.max_bytes:
+                    break
+                batch.append((m, sid))
+                nbytes += len(m)
+                i += 1
+            if not batch:
+                continue
+            data, off = pack_packets([m for m, _ in batch])
+            res = self._answers(lambda d, o, tcp: self.resolver.resolve_batch(d, o, seed=seed, qidx_base=qidx, tcp=tcp), data, off)
+            qidx += len(batch)
+            for _, sid in batch:
+                self.sessions[sid].queued -= 1
+            if res is None:
+                c['failed'] += len(batch)
+                continue
+            out, out_off, out_len, status, _ = res
+            for k, (m, sid) in enumerate(batch):
+                s = self.sessions[sid]
+                if status[k] == 0:
+                    c['answered'] += 1
+                    s.out += TcpFramer.frame(out[out_off[k]:out_off[k] + out_len[k]].tobytes())
+                elif status[k] == 1:
+                    c['missed'] += 1
+                    s.relays += 1
+                    misses.append((m, sid))
+                else:
+                    c['dropped'] += 1
+        return misses
+
+    def relay(self, queries, upstreams, sids):
+        """Replies to misses: query i answered from upstream response i (b'' = the lookup failed), appended to sids[i]."""
+        c = self.counters
+        for k0 in range(0, len(sids), self.max_batch):
+            qs, us, ss = queries[k0:k0 + self.max_batch], upstreams[k0:k0 + self.max_batch], sids[k0:k0 + self.max_batch]
+            res = self._answers(self.relayer.relay_batch, *(pack_packets(qs) + pack_packets(us)))
+            for j, sid in enumerate(ss):
+                s = self.sessions.get(sid)
+                if s is not None and s.relays:
+                    s.relays -= 1
+                if res is None:
+                    c['failed'] += 1
+                elif s is None or res[3][j] != 0:
+                    c['dropped'] += 1
+                else:
+                    out, out_off, out_len, _ = res
+                    s.out += TcpFramer.frame(out[out_off[j]:out_off[j] + out_len[j]].tobytes())
+                    c['relayed'] += 1
+
+    def output(self, sid):
+        s = self._get(sid)
+        return bytes(s.out), (s.eof or s.bad) and not s.queued and not s.relays and not s.out
+
+    def consume(self, sid, n):
+        s = self._get(sid)
+        if n > len(s.out):
+            raise ValueError('consume(%d) past the %d bytes of output' % (n, len(s.out)))
+        del s.out[:n]
+
+    def close(self, sid):
+        self._get(sid)
+        del self.sessions[sid]
+
+    def peer(self, sid):
+        s = self._get(sid)
+        return s.ip, s.port
+
+    def stats(self):
+        return dict(self.counters, open=len(self.sessions), queued=len(self.queue))
+
+
+class NativeTcpHub(object):
+    """bb_tcp_hub: TCP proxy sessions in the C library, their messages resolved as TCP batches on the engine.  Same
+    methods as TcpHub; argument errors (unknown or closed session, a closed hub) raise BinderError.  A failed batch is
+    counted, not raised: its code is in last_rc.  `lib` is the library to call (libbinder_b200.so by default)."""
+
+    def __init__(self, engine, max_batch=4096, lib=None):
+        import ctypes
+        from ._lib import BinderError, lib as _lib
+        self._L = lib if lib is not None else _lib()
+        err = ctypes.c_int(0)
+        self._h = self._L.bb_tcp_hub_create(engine._h, max_batch, ctypes.byref(err))
+        if not self._h:
+            raise BinderError(err.value)
+        self._engine, self.last_rc = engine, 0
+
+    def open(self):
+        import ctypes
+        from ._lib import check
+        sid = ctypes.c_uint32(0)
+        check(self._L.bb_tcp_hub_open(self._h, ctypes.byref(sid)))
+        return sid.value
+
+    def feed(self, sid, chunk):
+        from ._lib import check
+        chunk = bytes(chunk)
+        rc = self._L.bb_tcp_hub_feed(self._h, sid, chunk, len(chunk))
+        if rc == -8:
+            return False
+        check(rc)
+        return True
+
+    def eof(self, sid):
+        from ._lib import check
+        check(self._L.bb_tcp_hub_eof(self._h, sid))
+
+    def flush(self, seed):
+        import ctypes
+        from ._lib import check
+
+        class Misses(ctypes.Structure):
+            _fields_ = [('n', ctypes.c_uint32), ('pkts', ctypes.POINTER(ctypes.c_uint8)), ('pkt_off', ctypes.POINTER(ctypes.c_uint32)),
+                        ('session', ctypes.POINTER(ctypes.c_uint32))]
+        if not self._h:
+            check(-1)
+        m = Misses()
+        self.last_rc = self._L.bb_tcp_hub_flush(self._h, seed, ctypes.byref(m))
+        if m.n == 0:
+            return []
+        base = ctypes.addressof(m.pkts.contents)
+        return [(ctypes.string_at(base + m.pkt_off[i], m.pkt_off[i + 1] - m.pkt_off[i]), int(m.session[i])) for i in range(m.n)]
+
+    def relay(self, queries, upstreams, sids):
+        if not self._h:
+            from ._lib import check
+            check(-1)
+        (qd, qo), (ud, uo) = pack_packets(queries), pack_packets(upstreams)
+        s = np.ascontiguousarray(sids, dtype=np.uint32)
+        self.last_rc = self._L.bb_tcp_hub_relay(self._h, qd.ctypes.data, qo.ctypes.data, ud.ctypes.data, uo.ctypes.data,
+                                                s.ctypes.data if s.size else None, len(s))
+
+    def output(self, sid):
+        import ctypes
+        from ._lib import check
+        p, n, cl = ctypes.POINTER(ctypes.c_uint8)(), ctypes.c_size_t(0), ctypes.c_int(0)
+        check(self._L.bb_tcp_hub_output(self._h, sid, ctypes.byref(p), ctypes.byref(n), ctypes.byref(cl)))
+        return (ctypes.string_at(p, n.value) if n.value else b''), bool(cl.value)
+
+    def consume(self, sid, n):
+        from ._lib import check
+        check(self._L.bb_tcp_hub_consume(self._h, sid, n))
+
+    def close(self, sid):
+        from ._lib import check
+        check(self._L.bb_tcp_hub_close(self._h, sid))
+
+    def peer(self, sid):
+        import ctypes
+        from ._lib import check
+        ip, port = ctypes.c_uint32(0), ctypes.c_uint32(0)
+        check(self._L.bb_tcp_hub_peer(self._h, sid, ctypes.byref(ip), ctypes.byref(port)))
+        return ip.value, port.value
+
+    def stats(self):
+        st = {k: int(self._L.bb_tcp_hub_stat(self._h, i)) for i, k in enumerate(HUB_STATS)}
+        st['answer_capacity'] = int(self._L.bb_tcp_hub_stat(self._h, len(HUB_STATS)))
+        return st
+
+    def destroy(self):
+        if getattr(self, '_h', None):
+            self._L.bb_tcp_hub_destroy(self._h)
+            self._h = None
+
+    def __del__(self):
+        try:
+            self.destroy()
         except Exception:
             pass

@@ -32,7 +32,8 @@ enum {
     BB_ERR_CAPACITY = -5,   /* out_cap too small for this batch's responses              */
     BB_ERR_NO_DEVICE = -6,  /* no CUDA device: there is NO CPU fallback                   */
     BB_ERR_DOMAIN = -7,     /* dns_domain is not an encodable DNS name                   */
-    BB_ERR_PROTOCOL = -8    /* balancer frame stream: unknown type, INBOUND_TCP, oversized packet */
+    BB_ERR_PROTOCOL = -8    /* balancer frame stream: unknown type, INBOUND_TCP, oversized packet;
+                               TCP hub session: a first frame other than INBOUND_TCP, a zero-length message */
 };
 const char* bb_strerror(int err);
 const char* bb_last_cuda_error(void);
@@ -387,6 +388,59 @@ void        bb_backend_destroy(bb_backend* b);
 int         bb_backend_feed(bb_backend* b, const uint8_t* in, size_t in_len, uint64_t shuffle_seed,
                             const uint8_t** out, size_t* out_len, bb_backend_misses* misses);
 uint64_t    bb_backend_stat(const bb_backend* b, int what);   /* 0 udp frames 1 answered 2 missed 3 dropped 4 pending bytes 5 queries of failed batches */
+
+/* ---- mname-balancer TCP proxy sessions (deps/mname-balancer/backend.c:22-113, tcp_proxy.c:160-300) ----------------
+ * The balancer hands every DNS-over-TCP client connection to a backend as its own AF_UNIX session.  The session opens
+ * with INBOUND_TCP {3, src ip, src port} (12 bytes, u32 little-endian); the backend answers INBOUND_TCP_OK (u32 1003), its
+ * last frame on that session, and from then on the session carries the client's raw DNS-over-TCP stream both ways
+ * (2-byte big-endian length prefixes, RFC 1035 4.2.2).  A host routes a new AF_UNIX connection by its first frame:
+ * CLIENT_HELLO goes to a bb_backend, INBOUND_TCP to a TCP hub.  A hub owns many such sessions of one engine; the messages
+ * that complete on ALL of them between two flushes are resolved together.
+ *   create   max_batch is clamped to the engine's limits; query bytes per batch: max(64 x max_batch, 65,536), at most
+ *            the engine's max_batch_bytes (a message larger than that is dropped).  Answer bytes per batch (stat 10):
+ *            16 KB x max_batch, at least 1 MB, at most the engine's own response buffer (512 x its max_batch, >= 1 MB).
+ *   open     a new session; ids are not reused.
+ *   feed     bytes read from the session.  Before the handshake only a complete INBOUND_TCP frame is accepted: it records
+ *            the source address and queues INBOUND_TCP_OK as the session's first output.  Any other first frame, and a
+ *            zero-length DNS message later, is BB_ERR_PROTOCOL for this session only: it reads nothing more, messages
+ *            that completed before the error are still answered, and the session may close once they are written.
+ *            BB_ERR_ARG for a session that is unknown, closed, or past eof.
+ *   eof      the peer half-closed: complete messages are still answered, a partial one is discarded.
+ *   flush    every message completed since the last flush, in arrival order, through bb_resolve_batch_ex(BB_BATCH_TCP) in
+ *            batches split at max_batch or the query-byte limit; qidx_base runs 0, n0, n0 + n1, ... over the batches of
+ *            one flush.  Each answer is appended, length-prefixed, to its session's output: per session in arrival order.
+ *            Misses (BB_MISS_RECURSE) come back in *misses (packets + session ids, valid until the next flush) and stay
+ *            owed until relayed.  A failed batch (capacity, CUDA) loses its queries, counts them, and the flush goes on
+ *            with the next batch; the return value is then the first batch's error.
+ *   output   the bytes to write to the session (valid until the next hub call that changes it) and whether the session
+ *            may be closed: eof or protocol error seen, no message queued or owed a relay, nothing left to write.
+ *   consume  n bytes of that output were written.
+ *   close    forget the session; its queued messages and outstanding relays are dropped (counted).
+ *   relay    the host's upstream responses for misses (q = the miss packets, up = upstream i, empty = the lookup failed)
+ *            through bb_relay_batch(BB_BATCH_TCP), each reply appended length-prefixed to sessions[i]: RFC 7766 allows
+ *            out-of-order answers and the ID matches them.  Batches of max_batch; a failed one is counted as in flush.
+ */
+typedef struct bb_tcp_hub bb_tcp_hub;
+typedef struct bb_tcp_hub_misses {
+    uint32_t n; const uint8_t* pkts; const uint32_t* pkt_off /* n+1 */; const uint32_t* session;
+} bb_tcp_hub_misses;
+bb_tcp_hub* bb_tcp_hub_create(bb_engine* e, uint32_t max_batch, int* err);
+void        bb_tcp_hub_destroy(bb_tcp_hub* h);
+int         bb_tcp_hub_open(bb_tcp_hub* h, uint32_t* session);
+int         bb_tcp_hub_feed(bb_tcp_hub* h, uint32_t session, const uint8_t* in, size_t in_len);
+int         bb_tcp_hub_eof(bb_tcp_hub* h, uint32_t session);
+int         bb_tcp_hub_flush(bb_tcp_hub* h, uint64_t shuffle_seed, bb_tcp_hub_misses* misses);
+int         bb_tcp_hub_output(bb_tcp_hub* h, uint32_t session, const uint8_t** out, size_t* out_len, int* closable);
+int         bb_tcp_hub_consume(bb_tcp_hub* h, uint32_t session, size_t n);
+int         bb_tcp_hub_close(bb_tcp_hub* h, uint32_t session);
+int         bb_tcp_hub_relay(bb_tcp_hub* h, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* up_pkts,
+                             const uint32_t* up_off, const uint32_t* sessions, uint32_t n);
+/* the client's address from the session's INBOUND_TCP frame (0, 0 before the handshake) */
+int         bb_tcp_hub_peer(const bb_tcp_hub* h, uint32_t session, uint32_t* ip, uint32_t* port);
+/* 0 sessions opened 1 DNS messages received 2 answered 3 missed 4 dropped (undecodable, oversized, or of a closed session)
+ * 5 protocol errors 6 queries of failed batches 7 relay replies appended 8 sessions open 9 messages queued for the next flush
+ * 10 answer bytes per batch */
+uint64_t    bb_tcp_hub_stat(const bb_tcp_hub* h, int what);
 
 /* pinned host memory for the batch containers */
 void* bb_host_alloc(size_t bytes);
