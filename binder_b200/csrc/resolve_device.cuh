@@ -262,7 +262,7 @@ struct SvcView {
     __device__ uint32_t sp_len() const { return (h1.x >> 8) & 0xFF; }
     __device__ uint32_t dom_wl() const { return (h1.x >> 16) & 0xFF; }
     __device__ uint32_t srv_stride() const { return (h1.w >> 16) << 4; }
-    __device__ uint32_t add_stride() const { return ((h1.x & 0xFF) >> SVC_ADD_STRIDE_SHIFT) << 4; }
+    __device__ uint32_t add_stride() const { return svc_add_stride(h1.x); }
     __device__ uint32_t a_off() const { return svc_a_off(nkids()); }
     __device__ uint32_t rec_off() const { return svc_rec_off(nkids()); }
     __device__ uint32_t add_off() const { return svc_add_off(nkids()); }

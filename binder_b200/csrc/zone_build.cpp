@@ -659,9 +659,10 @@ bool emit_forward(bb_zone& zn, uint32_t id) {
             if (((ad.size() + 15) & ~(size_t)15) > add_stride) add_stride = (ad.size() + 15) & ~(size_t)15;
             if (((sr.size() + 15) & ~(size_t)15) > srv_stride) srv_stride = (sr.size() + 15) & ~(size_t)15;
         }
-        if (srv_stride / 16 > 0xFFFF || add_stride / 16 > 15) return false;
+        if (srv_stride / 16 > 0xFFFF || add_stride > SVC_ADD_STRIDE_MAX) return false;
+        if (add_stride > 240) add_stride = SVC_ADD_STRIDE_MAX;          // the one stride over 15 units the header can name
         h.stride16 = (uint16_t)(srv_stride / 16);
-        h.hflags |= (uint8_t)((add_stride / 16) << SVC_ADD_STRIDE_SHIFT);
+        h.hflags |= (uint8_t)svc_add_stride_bits((uint32_t)add_stride);
         // sums the kernel sizes an answer from without walking the children; a service too large for them is walked
         if (n_valid > 0xFFFF || sum_ports > 0xFFFF || sum_wl > 0xFFFF || sum_wl_ports > 0xFFFF || jobs_srv > 0xFFFF) h.hflags |= SVC_BAD_A | SVC_BAD_SRV;
         h.n_valid = (uint16_t)n_valid; h.sum_ports = (uint16_t)sum_ports; h.sum_wl = (uint16_t)sum_wl; h.sum_wl_ports = (uint16_t)sum_wl_ports;
@@ -1013,7 +1014,7 @@ extern "C" int bb_zone_probe(const bb_zone* z, uint32_t ns, const uint8_t* key, 
         std::string ext;
         if (h.hflags & bb::SVC_SP_EXT) { uint32_t off; memcpy(&off, h.sp, 4); ext.assign((const char*)A + off, h.sp_len); memset(h.sp, 0, 4); }
         out.append((const char*)&h, sizeof h); out += ext;                 // offsets are relative to the record: position independent
-        const size_t body = bb::svc_record_len(h.nkids, (uint32_t)(h.hflags >> bb::SVC_ADD_STRIDE_SHIFT) * 16, (uint32_t)h.stride16 * 16) - sizeof h;
+        const size_t body = bb::svc_record_len(h.nkids, bb::svc_add_stride(h.hflags), (uint32_t)h.stride16 * 16) - sizeof h;
         out.append((const char*)(A + s.val + sizeof h), body);
     } else if (s.kind == bb::K_PTR) {
         out.append((const char*)(A + s.val + 1), A[s.val]);

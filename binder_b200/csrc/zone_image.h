@@ -96,7 +96,17 @@ enum : uint8_t {
     SVC_SP_NEVER = 4,    // s.srvce / s.proto absent, not strings, or not spellable as labels: never equal (:334-335)
     SVC_SP_EXT = 8,      // the two labels do not fit `sp`: sp[0..3] = arena offset of the bytes
 };
-constexpr uint32_t SVC_ADD_STRIDE_SHIFT = 4;       // hflags >> 4: additional-section stride / 16 (1..5: a label is at most 63 bytes)
+// hflags >> 4: additional-section stride / 16.  A child is a znode path component and may contain dots, so its wire name is
+// up to 255 - dom_wl <= 252 bytes (several labels) and its additional RR (wire name + 16) up to 268: a stride of 1..17 units.
+// Four bits hold 1..15 as the count; 0 is never a count and stands for 17 (272 bytes), the stride of every child whose
+// additional RR is over 240 bytes.
+constexpr uint32_t SVC_ADD_STRIDE_SHIFT = 4;
+constexpr uint32_t SVC_ADD_STRIDE_MAX = 272;
+BB_HD uint32_t svc_add_stride(uint32_t hflags) {       // min(u - 1, 16) + 1 units: 0 wraps to 17 (an unsigned min, no branch)
+    const uint32_t m = ((hflags & 0xFF) >> SVC_ADD_STRIDE_SHIFT) - 1u;
+    return ((m < 16u ? m : 16u) + 1u) << 4;
+}
+BB_HD uint32_t svc_add_stride_bits(uint32_t stride) { return stride > 240 ? 0u : (stride >> 4) << SVC_ADD_STRIDE_SHIFT; }   // stride: 16..240 or 272
 struct alignas(32) SvcHdr {
     uint32_t ttl;            // after record.ttl / service.ttl / service.service.ttl (:270-274,331-332)
     uint16_t nkids;          // children that pass the type filter (:352-360), in child order
@@ -105,7 +115,7 @@ struct alignas(32) SvcHdr {
     uint16_t sum_wl;         // sum of wire_len over them
     uint16_t sum_wl_ports;   // sum of nports * wire_len over them
     uint16_t jobs_srv;       // copy jobs of a whole SRV answer (resolve_device.cuh: a piece is ceil(len / 64) jobs), OPT not counted
-    uint8_t  hflags;         // SVC_* | bytes per child of the additional section / 16 << 4 (SVC_ADD_STRIDE_SHIFT)
+    uint8_t  hflags;         // SVC_* | bytes per child of the additional section, encoded by svc_add_stride_bits
     uint8_t  sp_len;         // bytes of "_srvce._proto." on the wire = where the domain part of a matching SRV QNAME starts
     uint8_t  dom_wl;         // the service's fqdn as wire labels + terminator (what every SRV target ends with)
     uint8_t  sp[11];         // len, srvce bytes, len, proto bytes — as the query spells them
