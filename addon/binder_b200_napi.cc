@@ -182,6 +182,82 @@ static napi_value RelayBatch(napi_env env, napi_callback_info info) {
     return res;
 }
 
+// engineSetRecursionUpstreams(engine, ip: Uint32Array, port: Uint16Array, dc: Uint8Array)   (bb_engine_set_recursion_upstreams;
+//   ip and port in host byte order, dc = index in the filter's datacenter list)
+static napi_value EngineSetRecursionUpstreams(napi_env env, napi_callback_info info) {
+    size_t argc = 4; napi_value argv[4];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* e; NAPI_OK(napi_get_value_external(env, argv[0], &e));
+    napi_typedarray_type t1, t2, t3; size_t n1, n2, n3; void *p1, *p2, *p3; napi_value ab; size_t bo;
+    NAPI_OK(napi_get_typedarray_info(env, argv[1], &t1, &n1, &p1, &ab, &bo));
+    NAPI_OK(napi_get_typedarray_info(env, argv[2], &t2, &n2, &p2, &ab, &bo));
+    NAPI_OK(napi_get_typedarray_info(env, argv[3], &t3, &n3, &p3, &ab, &bo));
+    if (t1 != napi_uint32_array || t2 != napi_uint16_array || t3 != napi_uint8_array || n1 != n2 || n1 != n3) return Throw(env, BB_ERR_ARG);
+    int rc = bb_engine_set_recursion_upstreams((bb_engine*)e, (const uint32_t*)p1, (const uint16_t*)p2, (const uint8_t*)p3, (uint32_t)n1);
+    if (rc != BB_OK) return Throw(env, rc);
+    return nullptr;
+}
+
+// forwardBatch(engine, pkts: Buffer, pktOff: Uint32Array(n+1), idKey: BigInt)
+//   -> {uq: Buffer, uqOff: Uint32Array(n+1), order: Uint32Array(n), groupOff: Uint32Array(19), route: Uint8Array(n)}:
+//   the upstream queries of the misses, grouped by datacenter (bb_forward_batch); draw a fresh idKey for every call
+static napi_value ForwardBatch(napi_env env, napi_callback_info info) {
+    size_t argc = 4; napi_value argv[4];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* e; NAPI_OK(napi_get_value_external(env, argv[0], &e));
+    void* pk; size_t pklen; NAPI_OK(napi_get_buffer_info(env, argv[1], &pk, &pklen));
+    const uint32_t* po; size_t pn;
+    if (!check_off(env, argv[2], pklen, &po, &pn) || pn - 1 > BB_FORWARD_MAX) return Throw(env, BB_ERR_ARG);
+    uint64_t key = 0; bool lossless; NAPI_OK(napi_get_value_bigint_uint64(env, argv[3], &key, &lossless));
+    const uint32_t n = (uint32_t)pn - 1, cap = po[n];
+    void *uq, *uo, *od, *go, *rt; napi_value b_uq, a_uo, a_od, a_go, a_rt, t_uo, t_od, t_go, t_rt;
+    NAPI_OK(napi_create_buffer(env, cap ? cap : 1, &uq, &b_uq));
+    NAPI_OK(napi_create_arraybuffer(env, (n + 1) * 4, &uo, &a_uo)); NAPI_OK(napi_create_typedarray(env, napi_uint32_array, n + 1, a_uo, 0, &t_uo));
+    NAPI_OK(napi_create_arraybuffer(env, n * 4, &od, &a_od));       NAPI_OK(napi_create_typedarray(env, napi_uint32_array, n, a_od, 0, &t_od));
+    NAPI_OK(napi_create_arraybuffer(env, (BB_ROUTE_NONE + 2) * 4, &go, &a_go));
+    NAPI_OK(napi_create_typedarray(env, napi_uint32_array, BB_ROUTE_NONE + 2, a_go, 0, &t_go));
+    NAPI_OK(napi_create_arraybuffer(env, n, &rt, &a_rt));           NAPI_OK(napi_create_typedarray(env, napi_uint8_array, n, a_rt, 0, &t_rt));
+    int rc = bb_forward_batch((bb_engine*)e, (const uint8_t*)pk, po, n, key, (uint8_t*)uq, cap, (uint32_t*)uo, (uint32_t*)od, (uint32_t*)go,
+                              (uint8_t*)rt);
+    if (rc != BB_OK) return Throw(env, rc);
+    napi_value res; NAPI_OK(napi_create_object(env, &res));
+    napi_set_named_property(env, res, "uq", b_uq);         napi_set_named_property(env, res, "uqOff", t_uo);
+    napi_set_named_property(env, res, "order", t_od);      napi_set_named_property(env, res, "groupOff", t_go);
+    napi_set_named_property(env, res, "route", t_rt);
+    return res;
+}
+
+// matchUpstreams(engine, resp: Buffer, respOff: Uint32Array(m+1), srcIp: Uint32Array(m), srcPort: Uint16Array(m),
+//                pkts: Buffer, pktOff: Uint32Array(n+1), route: Uint8Array(n), idKey: BigInt)
+//   -> {up: Buffer, upOff: Uint32Array(n+1)}: each miss's accepted upstream response, relayBatch's upstream input
+//   (bb_match_upstreams); pkts / route are the forwardBatch call's misses and routes, in miss order
+static napi_value MatchUpstreams(napi_env env, napi_callback_info info) {
+    size_t argc = 9; napi_value argv[9];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* e; NAPI_OK(napi_get_value_external(env, argv[0], &e));
+    void* rs; size_t rslen; NAPI_OK(napi_get_buffer_info(env, argv[1], &rs, &rslen));
+    void* pk; size_t pklen; NAPI_OK(napi_get_buffer_info(env, argv[5], &pk, &pklen));
+    const uint32_t *ro, *po; size_t rn, pn;
+    if (!check_off(env, argv[2], rslen, &ro, &rn) || !check_off(env, argv[6], pklen, &po, &pn)) return Throw(env, BB_ERR_ARG);
+    napi_typedarray_type ti, tp, tr; size_t ni, np_, nr; void *pi, *pp, *pr; napi_value ab; size_t bo;
+    NAPI_OK(napi_get_typedarray_info(env, argv[3], &ti, &ni, &pi, &ab, &bo));
+    NAPI_OK(napi_get_typedarray_info(env, argv[4], &tp, &np_, &pp, &ab, &bo));
+    NAPI_OK(napi_get_typedarray_info(env, argv[7], &tr, &nr, &pr, &ab, &bo));
+    if (ti != napi_uint32_array || tp != napi_uint16_array || tr != napi_uint8_array || ni != rn - 1 || np_ != rn - 1 || nr != pn - 1)
+        return Throw(env, BB_ERR_ARG);
+    uint64_t key = 0; bool lossless; NAPI_OK(napi_get_value_bigint_uint64(env, argv[8], &key, &lossless));
+    const uint32_t m = (uint32_t)rn - 1, n = (uint32_t)pn - 1, cap = ro[m];
+    void *up, *uo; napi_value b_up, a_uo, t_uo;
+    NAPI_OK(napi_create_buffer(env, cap ? cap : 1, &up, &b_up));
+    NAPI_OK(napi_create_arraybuffer(env, (n + 1) * 4, &uo, &a_uo)); NAPI_OK(napi_create_typedarray(env, napi_uint32_array, n + 1, a_uo, 0, &t_uo));
+    int rc = bb_match_upstreams((bb_engine*)e, (const uint8_t*)rs, ro, (const uint32_t*)pi, (const uint16_t*)pp, m, (const uint8_t*)pk, po,
+                                (const uint8_t*)pr, n, key, (uint8_t*)up, cap, (uint32_t*)uo);
+    if (rc != BB_OK) return Throw(env, rc);
+    napi_value res; NAPI_OK(napi_create_object(env, &res));
+    napi_set_named_property(env, res, "up", b_up); napi_set_named_property(env, res, "upOff", t_uo);
+    return res;
+}
+
 // ---- TCP proxy sessions from mname-balancer (bb_tcp_hub): route a new AF_UNIX connection whose first frame is
 // INBOUND_TCP here.  Session ids travel as Uint32Array(1), counters as BigUint64Array.
 //   tcpHubCreate(engine, maxBatch) -> hub          tcpHubOpen(hub) -> Uint32Array [session]
@@ -325,6 +401,9 @@ static napi_value Init(napi_env env, napi_value exports) {
         { "engineSetRecursionFilter", nullptr, EngineSetRecursionFilter, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "resolveBatch", nullptr, ResolveBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "relayBatch", nullptr, RelayBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "engineSetRecursionUpstreams", nullptr, EngineSetRecursionUpstreams, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "forwardBatch", nullptr, ForwardBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "matchUpstreams", nullptr, MatchUpstreams, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "tcpHubCreate", nullptr, TcpHubCreate, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "tcpHubOpen", nullptr, TcpHubOpen, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "tcpHubFeed", nullptr, TcpHubFeed, nullptr, nullptr, nullptr, napi_default, nullptr },

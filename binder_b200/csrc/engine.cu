@@ -36,6 +36,7 @@ extern "C" uint64_t bb_zone_sync_gen(const bb_zone* z);
 
 #include "resolve_device.cuh"
 #include "relay_device.cuh"
+#include "forward_device.cuh"
 
 namespace bbk {
 // ---- the kernel ------------------------------------------------------------------------------
@@ -573,6 +574,213 @@ __global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
         });
 }
 
+// ---- recursion forward and match (DESIGN.md section 14, lib/recursion.js:253-280,335-354,382-387) ----------------------
+// Forward: three launches per call.  forward_kernel takes a tile of 128 misses, a thread per miss: decode, route, the
+// client query packed in miss order (CTA scan + look-back placement, the relay's input as it stands) and the tile's
+// histogram of (upstream queries, bytes) per route.  forward_group_kernel (one block) scans the histograms route-major
+// into every (tile, route)'s output base — the stable counting sort's scan.  forward_scatter_kernel ranks each miss
+// inside its tile's run of its route and writes its upstream query there.
+// Match: match_kernel, a thread per received datagram, keeps the earliest acceptable response per miss (atomicMin on
+// the arrival index); match_gather_kernel packs the winners in miss order (CTA scan + look-back) and resets the
+// winner table for the next call.
+struct FwdParams {
+    const uint8_t* pkts; const uint32_t* pkt_off;
+    const uint32_t* miss_idx;             // miss j = packet miss_idx[j]; NULL: miss j = packet j (packed misses, staged)
+    const uint32_t* n_dev;                // when set, the miss count is n_dev[1] (a resolve launch's totals)
+    uint32_t n, n_cap;                    // n_cap: misses the launch covers (more is an error)
+    const EngineConst* eng; IdKey key;
+    uint8_t* uq; uint32_t uq_cap; uint32_t* uq_off; uint32_t* order; uint32_t* group_off; uint8_t* route;
+    uint8_t* q; uint32_t q_cap; uint32_t* q_off;
+    uint32_t* totals;                     // {upstream bytes, n, error marker, done marker, client bytes}
+    unsigned long long* hist;             // [tile][route]: count << 32 | bytes, then the (tile, route) output base
+    uint16_t* ulen;                       // [j]: upstream query length
+    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap, epoch;
+};
+template <class PP>
+__device__ __forceinline__ uint32_t fwd_count(const PP& P, bool& bad) {
+    const uint32_t n = P.n_dev ? *(volatile const uint32_t*)(P.n_dev + 1) : P.n;
+    bad = n > P.n_cap;
+    return bad ? 0u : n;
+}
+
+__global__ void __launch_bounds__(T) forward_kernel(const FwdParams P) {
+    __shared__ __align__(16) uint8_t s_in[RS_Q + 32];
+    __shared__ uint32_t s_off[T + 1];
+    __shared__ uint32_t s_wsum[T / 32];
+    __shared__ uint32_t s_cnt[NROUTE], s_byt[NROUTE];
+    __shared__ unsigned long long s_prefix;
+    __shared__ __align__(8) unsigned long long s_bar;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    bool bad;
+    const uint32_t n = fwd_count(P, bad), tile = blockIdx.x, ntiles = (n + T - 1) / T;
+    if (tile < ntiles) {
+        const uint32_t j0 = tile * T, nq = min((uint32_t)T, n - j0), j = j0 + tid;
+        const bool packed = P.miss_idx == nullptr;
+        const uint32_t bar = (uint32_t)__cvta_generic_to_shared(&s_bar);
+        if (tid < (int)NROUTE) { s_cnt[tid] = 0; s_byt[tid] = 0; }
+        if (packed && tid == 0) { mbar_init(bar, 1); stage_range(bar, s_in, P.pkts, P.pkt_off[j0], P.pkt_off[j0 + nq], RS_Q); }
+        uint32_t o0 = 0, o1 = 0;
+        if (tid < (int)nq) { const uint32_t p = packed ? j : P.miss_idx[j]; o0 = P.pkt_off[p]; o1 = P.pkt_off[p + 1]; }
+        if (packed) { if (tid < (int)nq) s_off[tid] = o0; if (tid == 0) s_off[nq] = P.pkt_off[j0 + nq]; }
+        __syncthreads();
+        const uint32_t b0 = packed ? s_off[0] : 0u, b1 = packed ? s_off[nq] : 0u;
+        const bool staged = packed && stage_wait(bar, b0, b1, RS_Q);
+        // a packed miss must lie inside its tile's byte range; every miss is at most 65,535 bytes
+        uint32_t clen = 0, ul = 0, rt = RT_NONE;
+        const uint8_t* pk = nullptr;
+        if (tid < (int)nq && o1 >= o0 && o1 - o0 <= 65535u && (!packed || (o0 >= b0 && o1 <= b1))) {
+            clen = o1 - o0;
+            pk = staged ? s_in + (o0 - (b0 & ~15u)) : P.pkts + o0;
+            Res d;
+            if (decode(pk, clen, d)) { rt = fwd_route(P.eng, pk, d); ul = 12 + d.qn_len + 4; }
+        }
+        if (tid < (int)nq) { atomicAdd(&s_cnt[rt], 1u); atomicAdd(&s_byt[rt], ul); }
+        const TileScan sc = cta_scan<false>(clen, 0, s_wsum, nullptr, lane, warp);      // 128 x 65,535 < 2^24
+        const uint64_t base = place_tile<true>(P.desc, P.ntiles_cap, tile, sc.tot, 0, s_prefix, tid) & D_VAL;
+        const bool ovf = base + sc.tot > (uint64_t)P.q_cap;
+        if (tid < (int)nq) {
+            const uint32_t at = (uint32_t)(base + sc.ex);
+            P.q_off[j] = at; P.route[j] = (uint8_t)rt; P.ulen[j] = (uint16_t)ul;
+            if (!ovf) for (uint32_t i = 0; i < clen; i++) P.q[at + i] = pk[i];
+        }
+        if (ovf && tid == 0) P.totals[2] = P.epoch;
+        if (tid < (int)NROUTE) P.hist[(size_t)tile * NROUTE + tid] = (unsigned long long)s_cnt[tid] << 32 | s_byt[tid];
+    }
+    if (warp == 0)
+        self_clean<true>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+            const uint32_t tb = (uint32_t)cur;
+            P.q_off[n] = tb; P.totals[4] = tb; P.totals[1] = n;
+            if (bad) P.totals[2] = P.epoch;
+        });
+}
+
+// One block of FWD_MAX / T threads, thread t = tile t: every (tile, route) histogram entry becomes that run's output
+// base (position << 32 | byte offset), route-major so that each route's upstream queries are one contiguous run.
+constexpr int FG_T = FWD_MAX / T;
+__global__ void __launch_bounds__(FG_T) forward_group_kernel(const FwdParams P) {
+    __shared__ unsigned long long s_w[FG_T / 32][NROUTE];
+    __shared__ unsigned long long s_rbase[NROUTE + 1];
+    const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+    bool bad;
+    const uint32_t n = fwd_count(P, bad), ntiles = (n + T - 1) / T;
+    unsigned long long incl[NROUTE];
+#pragma unroll
+    for (uint32_t r = 0; r < NROUTE; r++) {
+        unsigned long long x = t < (int)ntiles ? P.hist[(size_t)t * NROUTE + r] : 0ull;
+        for (int o = 1; o < 32; o <<= 1) { const unsigned long long y = __shfl_up_sync(0xffffffffu, x, o); if (lane >= o) x += y; }
+        incl[r] = x;
+        if (lane == 31) s_w[warp][r] = x;
+    }
+    __syncthreads();
+    if (t < (int)NROUTE) {
+        unsigned long long acc = 0;
+        for (int w = 0; w < FG_T / 32; w++) { const unsigned long long x = s_w[w][t]; s_w[w][t] = acc; acc += x; }
+        s_rbase[t] = acc;                                                   // the route's total, for now
+    }
+    __syncthreads();
+    if (t == 0) {
+        unsigned long long acc = 0;
+        for (uint32_t r = 0; r < NROUTE; r++) { const unsigned long long x = s_rbase[r]; s_rbase[r] = acc; acc += x; }
+        s_rbase[NROUTE] = acc;
+    }
+    __syncthreads();
+    if (t < (int)ntiles) {
+#pragma unroll
+        for (uint32_t r = 0; r < NROUTE; r++) {
+            const unsigned long long own = P.hist[(size_t)t * NROUTE + r];
+            P.hist[(size_t)t * NROUTE + r] = s_rbase[r] + s_w[warp][r] + incl[r] - own;
+        }
+    }
+    if (t <= (int)NROUTE) P.group_off[t] = (uint32_t)(s_rbase[t] >> 32);
+    if (t == 0) {
+        const uint32_t tb = (uint32_t)s_rbase[NROUTE];
+        P.uq_off[n] = tb; P.totals[0] = tb;
+        if (tb > P.uq_cap) P.totals[2] = P.epoch;
+        P.totals[3] = P.epoch;
+    }
+}
+
+__global__ void __launch_bounds__(T) forward_scatter_kernel(const FwdParams P) {
+    __shared__ uint8_t s_rt[T];
+    __shared__ uint16_t s_len[T];
+    __shared__ uint32_t s_rank[T], s_boff[T];
+    const int tid = threadIdx.x;
+    bool bad;
+    const uint32_t n = fwd_count(P, bad), tile = blockIdx.x, ntiles = (n + T - 1) / T;
+    if (tile >= ntiles || *(volatile const uint32_t*)(P.totals + 2) == P.epoch) return;     // nothing to place, or it does not fit
+    const uint32_t j0 = tile * T, nq = min((uint32_t)T, n - j0), j = j0 + tid;
+    if (tid < (int)nq) { s_rt[tid] = P.route[j]; s_len[tid] = P.ulen[j]; }
+    __syncthreads();
+    // stable rank inside the tile: thread r walks the tile's misses in order and numbers those of route r
+    if (tid < (int)NROUTE) {
+        uint32_t c = 0, b = 0;
+        for (uint32_t i = 0; i < nq; i++) if (s_rt[i] == tid) { s_rank[i] = c++; s_boff[i] = b; b += s_len[i]; }
+    }
+    __syncthreads();
+    if (tid < (int)nq) {
+        const unsigned long long base = P.hist[(size_t)tile * NROUTE + s_rt[tid]];
+        const uint32_t pos = (uint32_t)(base >> 32) + s_rank[tid], at = (uint32_t)base + s_boff[tid];
+        P.order[pos] = j; P.uq_off[pos] = at;
+        if (s_len[tid]) fwd_emit(P.q + P.q_off[j], s_len[tid] - 16u, id_enc(P.key, j), P.uq + at);
+    }
+}
+
+struct MatchParams {
+    const uint8_t* resp; const uint32_t* resp_off; const uint32_t* src_ip; const uint16_t* src_port; uint32_t n_resp;
+    const uint8_t* c; const uint32_t* c_off; const uint8_t* route;
+    const uint32_t* n_dev; uint32_t n, n_cap;         // n_dev: the forward launch's totals (n = n_dev[1])
+    const EngineConst* eng; IdKey key;
+    uint32_t* win;                                    // [j]: earliest accepted arrival index (NO_MATCH between calls)
+    uint8_t* up; uint32_t up_cap; uint32_t* up_off;
+    uint32_t* totals;                                 // {response bytes, misses answered, overflow marker, done marker}
+    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap, epoch;
+};
+
+__global__ void __launch_bounds__(256) match_kernel(const MatchParams P) {
+    const uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
+    if (r >= P.n_resp) return;
+    bool bad;
+    const uint32_t n = fwd_count(P, bad);
+    const uint32_t u0 = P.resp_off[r], u1 = P.resp_off[r + 1];
+    if (u1 < u0) return;
+    const uint32_t j = match_one(P.eng, P.key, P.resp + u0, u1 - u0, P.src_ip[r], P.src_port[r], n, P.route, P.c, P.c_off);
+    if (j != NO_MATCH) atomicMin(P.win + j, r);
+}
+
+__global__ void __launch_bounds__(T) match_gather_kernel(const MatchParams P) {
+    __shared__ uint32_t s_wsum[T / 32], s_wsum2[T / 32];
+    __shared__ unsigned long long s_prefix;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    bool bad;
+    const uint32_t n = fwd_count(P, bad), tile = blockIdx.x, ntiles = (n + T - 1) / T;
+    if (tile < ntiles) {
+        const uint32_t j0 = tile * T, nq = min((uint32_t)T, n - j0), j = j0 + tid;
+        uint32_t w = NO_MATCH, len = 0;
+        if (tid < (int)nq) {
+            w = P.win[j];
+            P.win[j] = NO_MATCH;                                          // ready for the next call
+            if (w != NO_MATCH) len = P.resp_off[w + 1] - P.resp_off[w];   // accepted: offsets in order, length >= 12
+            if (len > 65535u) { len = 0; w = NO_MATCH; }
+        }
+        const TileScan sc = cta_scan<true>(len, w != NO_MATCH ? 1u : 0u, s_wsum, s_wsum2, lane, warp);
+        const uint64_t ex = place_tile<true>(P.desc, P.ntiles_cap, tile, sc.tot, sc.tot2, s_prefix, tid);
+        const uint64_t base = ex & ((1ull << D_MISS_SHIFT) - 1);
+        const bool ovf = base + sc.tot > (uint64_t)P.up_cap;
+        if (tid < (int)nq) {
+            const uint32_t at = (uint32_t)(base + sc.ex);
+            P.up_off[j] = at;
+            if (!ovf && len) { const uint8_t* src = P.resp + P.resp_off[w]; for (uint32_t i = 0; i < len; i++) P.up[at + i] = src[i]; }
+        }
+        if (ovf && tid == 0) P.totals[2] = P.epoch;
+    }
+    if (warp == 0)
+        self_clean<true>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+            const uint32_t tb = (uint32_t)(cur & ((1ull << D_MISS_SHIFT) - 1));
+            P.up_off[n] = tb; P.totals[0] = tb; P.totals[1] = (uint32_t)(cur >> D_MISS_SHIFT); P.totals[3] = P.epoch;
+            if (bad) P.totals[2] = P.epoch;
+        });
+}
+
 // ---- multi-GPU: route + push ----------------------------------------------------------------
 // Ingress side of the sharded design (SURVEY.md §8e).  Each query is parsed just far enough to
 // know its lookup key (the same code as resolve, in route mode) and is then written straight
@@ -841,6 +1049,12 @@ struct bb_engine {
     struct RelayBuf { void* p = nullptr; size_t cap = 0; };
     RelayBuf r_q, r_qoff, r_up, r_upoff, r_out, r_out_off, r_out_len, r_status, r_totals;
     PinnedCheck r_pinned;                        // of bb_relay_batch's output sets
+    // forward / match scratch (per-tile histograms, upstream query lengths, the match's winner table), one per stream
+    // like the look-back scratch: [MAX_DEV_STREAMS] = the synchronous calls' (slot 0's stream)
+    struct FwdScratch { unsigned long long* hist = nullptr; uint16_t* ulen = nullptr; uint32_t* win = nullptr; };
+    FwdScratch fwd[MAX_DEV_STREAMS + 1];
+    // bb_forward_batch / bb_match_upstreams device staging
+    RelayBuf f_pk, f_pkoff, f_uq, f_uqoff, f_order, f_goff, f_route, f_q, f_qoff, f_tot, f_resp, f_respoff, f_ip, f_port, f_up, f_upoff;
 };
 
 // The zone and engine fields of the kernel parameters
@@ -955,6 +1169,10 @@ void bb_engine_destroy(bb_engine* e) {
     for (int i = 0; i < e->n_dev_streams; i++) cudaFree(e->dev_desc[i]);
     for (auto* b : { &e->r_q, &e->r_qoff, &e->r_up, &e->r_upoff, &e->r_out, &e->r_out_off, &e->r_out_len, &e->r_status, &e->r_totals })
         cudaFree(b->p);
+    for (auto* b : { &e->f_pk, &e->f_pkoff, &e->f_uq, &e->f_uqoff, &e->f_order, &e->f_goff, &e->f_route, &e->f_q, &e->f_qoff,
+                     &e->f_tot, &e->f_resp, &e->f_respoff, &e->f_ip, &e->f_port, &e->f_up, &e->f_upoff })
+        cudaFree(b->p);
+    for (auto& f : e->fwd) { cudaFree(f.hist); cudaFree(f.ulen); cudaFree(f.win); }
     cudaFree(e->d_const); cudaFree(e->d_table); cudaFree(e->d_arena);
     if (e->h_fb) cudaFreeHost(e->h_fb);
     delete e;
@@ -1028,6 +1246,18 @@ int bb_engine_set_recursion_filter(bb_engine* e, const char* region_domain, cons
     if (!bb::set_recursion_filter_const(e->hconst, region_domain, dc_names, n_dc, ptr_forwardable != 0)) return BB_ERR_ARG;
     CK(cudaSetDevice(e->device));
     CK(cudaDeviceSynchronize());                                   // batches in flight finish with the old filter
+    CK(cudaMemcpy(e->d_const, &e->hconst, sizeof(bb::EngineConst), cudaMemcpyHostToDevice));
+    return BB_OK;
+}
+// The upstream resolvers of the forward and match kernels (lib/recursion.js:205-240,360-379): entry i is ip[i]:port[i] of
+// the datacenter dc[i] of the filter's list.  Same synchronisation as the filter.
+int bb_engine_set_recursion_upstreams(bb_engine* e, const uint32_t* ip, const uint16_t* port, const uint8_t* dc, uint32_t n) {
+    if (!e) return BB_ERR_ARG;
+    bb::EngineConst c = e->hconst;
+    if (!bb::set_recursion_upstreams_const(c, ip, port, dc, n)) return BB_ERR_ARG;
+    CK(cudaSetDevice(e->device));
+    CK(cudaDeviceSynchronize());                                   // batches in flight finish with the old table
+    e->hconst = c;
     CK(cudaMemcpy(e->d_const, &e->hconst, sizeof(bb::EngineConst), cudaMemcpyHostToDevice));
     return BB_OK;
 }
@@ -1196,6 +1426,184 @@ int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t*
     if (rc != BB_OK) return rc;
     return relay_launch(e, desc, d_q_pkts, d_q_off, d_up_pkts, d_up_off, n, flags, d_out, out_cap, d_out_off, d_out_len, d_status,
                         d_totals, nullptr, (cudaStream_t)stream);
+}
+
+// ---- recursion forward and match (lib/recursion.js:253-280,335-354,382-387) --------------------------------------------
+static bool forward_ready(const bb_engine* e) { return e && e->hconst.recursion == 2 && e->hconst.fu_n; }
+// Look-back and forward scratch of `stream` (NULL `stream` with `sync`: the synchronous calls' own, on slot 0's stream).
+static int fwd_scratch(bb_engine* e, void* stream, bool sync, unsigned long long** desc, bb_engine::FwdScratch** fs) {
+    int si = bb_engine::MAX_DEV_STREAMS;
+    if (sync) *desc = e->slots[0].d_desc;
+    else {
+        int rc = stream_desc(e, stream, desc);
+        if (rc != BB_OK) return rc;
+        for (int i = 0; i < e->n_dev_streams; i++) if (e->dev_stream[i] == stream) si = i;
+    }
+    bb_engine::FwdScratch& f = e->fwd[si];
+    if (!f.hist) {
+        CK(cudaSetDevice(e->device));
+        CK(cudaMalloc(&f.hist, (size_t)(bbk::FWD_MAX / bbk::T) * bbk::NROUTE * 8));
+        CK(cudaMalloc(&f.ulen, (size_t)bbk::FWD_MAX * 2));
+        CK(cudaMalloc(&f.win, (size_t)bbk::FWD_MAX * 4));
+        CK(cudaMemset(f.win, 0xFF, (size_t)bbk::FWD_MAX * 4));       // NO_MATCH; match_gather_kernel leaves it so
+    }
+    *fs = &f;
+    return BB_OK;
+}
+// the misses one forward / match launch covers: the engine's look-back scratch holds max_tiles tiles
+static uint32_t fwd_cap(const bb_engine* e, uint32_t n_cap) {
+    return std::min(std::min(n_cap, bbk::FWD_MAX), e->max_tiles * (uint32_t)bbk::T);
+}
+
+static int forward_launch(bb_engine* e, unsigned long long* desc, bb_engine::FwdScratch* fs, const uint8_t* pkts, const uint32_t* pkt_off,
+                          const uint32_t* miss_idx, const uint32_t* n_dev, uint32_t n, uint32_t n_cap, uint64_t id_key,
+                          uint8_t* uq, uint32_t uq_cap, uint32_t* uq_off, uint32_t* order, uint32_t* group_off, uint8_t* route,
+                          uint8_t* q, uint32_t q_cap, uint32_t* q_off, uint32_t* totals, cudaStream_t st) {
+    bbk::FwdParams P;
+    P.pkts = pkts; P.pkt_off = pkt_off; P.miss_idx = miss_idx; P.n_dev = n_dev; P.n = n; P.n_cap = n_cap;
+    P.eng = e->d_const; P.key = bbk::id_key_rounds(id_key);
+    P.uq = uq; P.uq_cap = uq_cap; P.uq_off = uq_off; P.order = order; P.group_off = group_off; P.route = route;
+    P.q = q; P.q_cap = q_cap; P.q_off = q_off; P.totals = totals; P.hist = fs->hist; P.ulen = fs->ulen;
+    P.desc = desc; P.counter = (uint32_t*)(desc + e->max_tiles + 1); P.ntiles_cap = e->max_tiles;
+    P.epoch = (uint32_t)(++e->epoch);
+    const uint32_t ntiles = (n_cap + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;     // an empty call still reports its totals
+    bbk::forward_kernel<<<grid, bbk::T, 0, st>>>(P);
+    bbk::forward_group_kernel<<<1, bbk::FG_T, 0, st>>>(P);
+    bbk::forward_scatter_kernel<<<grid, bbk::T, 0, st>>>(P);
+    CK(cudaGetLastError());
+    e->launches += 3;
+    return BB_OK;
+}
+
+static int match_launch(bb_engine* e, unsigned long long* desc, bb_engine::FwdScratch* fs, const uint8_t* resp, const uint32_t* resp_off,
+                        const uint32_t* src_ip, const uint16_t* src_port, uint32_t n_resp, const uint8_t* q, const uint32_t* q_off,
+                        const uint8_t* route, const uint32_t* n_dev, uint32_t n, uint32_t n_cap, uint64_t id_key, uint8_t* up,
+                        uint32_t up_cap, uint32_t* up_off, uint32_t* totals, cudaStream_t st) {
+    bbk::MatchParams P;
+    P.resp = resp; P.resp_off = resp_off; P.src_ip = src_ip; P.src_port = src_port; P.n_resp = n_resp;
+    P.c = q; P.c_off = q_off; P.route = route; P.n_dev = n_dev; P.n = n; P.n_cap = n_cap;
+    P.eng = e->d_const; P.key = bbk::id_key_rounds(id_key); P.win = fs->win;
+    P.up = up; P.up_cap = up_cap; P.up_off = up_off; P.totals = totals;
+    P.desc = desc; P.counter = (uint32_t*)(desc + e->max_tiles + 1); P.ntiles_cap = e->max_tiles;
+    P.epoch = (uint32_t)(++e->epoch);
+    if (n_resp) bbk::match_kernel<<<(n_resp + 255) / 256, 256, 0, st>>>(P);
+    const uint32_t ntiles = (n_cap + bbk::T - 1) / bbk::T;
+    bbk::match_gather_kernel<<<ntiles ? ntiles : 1u, bbk::T, 0, st>>>(P);
+    CK(cudaGetLastError());
+    e->launches += n_resp ? 2 : 1;
+    return BB_OK;
+}
+
+static bool offsets_ok(const uint32_t* off, uint32_t n) {
+    for (uint32_t i = 0; i < n; i++) if (off[i + 1] < off[i]) return false;
+    return true;
+}
+
+int bb_forward_batch(bb_engine* e, const uint8_t* pkts, const uint32_t* pkt_off, uint32_t n, uint64_t id_key, uint8_t* uq,
+                     uint32_t uq_cap, uint32_t* uq_off, uint32_t* order, uint32_t* group_off, uint8_t* route) {
+    if (!forward_ready(e) || !pkt_off || !uq_off || !group_off || n > fwd_cap(e, bbk::FWD_MAX)) return BB_ERR_ARG;
+    if (n && (!order || !route || !uq || (pkt_off[n] && !pkts) || !offsets_ok(pkt_off, n))) return BB_ERR_ARG;
+    const uint32_t bytes = pkt_off[n];
+    CK(cudaSetDevice(e->device));
+    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
+    int rc;
+    if ((rc = fwd_scratch(e, nullptr, true, &desc, &fs)) || (rc = relay_grow(e->f_pk, (size_t)bytes + 64)) ||
+        (rc = relay_grow(e->f_pkoff, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->f_uq, (size_t)bytes + 64)) ||
+        (rc = relay_grow(e->f_uqoff, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->f_order, (size_t)n * 4 + 16)) ||
+        (rc = relay_grow(e->f_goff, (bbk::NROUTE + 1) * 4)) || (rc = relay_grow(e->f_route, (size_t)n + 16)) ||
+        (rc = relay_grow(e->f_q, (size_t)bytes + 64)) || (rc = relay_grow(e->f_qoff, ((size_t)n + 1) * 4)) ||
+        (rc = relay_grow(e->f_tot, 32)))
+        return rc;
+    cudaStream_t st = e->slots[0].stream;
+    if (bytes) CK(cudaMemcpyAsync(e->f_pk.p, pkts, bytes, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->f_pkoff.p, pkt_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
+    // an upstream query is never longer than its client query: the device buffers hold the whole batch
+    rc = forward_launch(e, desc, fs, (uint8_t*)e->f_pk.p, (uint32_t*)e->f_pkoff.p, nullptr, nullptr, n, n, id_key, (uint8_t*)e->f_uq.p,
+                        bytes, (uint32_t*)e->f_uqoff.p, (uint32_t*)e->f_order.p, (uint32_t*)e->f_goff.p, (uint8_t*)e->f_route.p,
+                        (uint8_t*)e->f_q.p, bytes, (uint32_t*)e->f_qoff.p, (uint32_t*)e->f_tot.p, st);
+    if (rc != BB_OK) return rc;
+    const uint32_t epoch = (uint32_t)e->epoch;
+    uint32_t tot[5];
+    CK(cudaMemcpyAsync(tot, e->f_tot.p, 20, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (tot[2] == epoch) { g_cuda_err = "forward: device buffers overflowed"; return BB_ERR_CUDA; }
+    if (tot[0] > uq_cap) return BB_ERR_CAPACITY;
+    if (tot[0]) CK(cudaMemcpyAsync(uq, e->f_uq.p, tot[0], cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(uq_off, e->f_uqoff.p, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(group_off, e->f_goff.p, (bbk::NROUTE + 1) * 4, cudaMemcpyDeviceToHost, st));
+    if (n) CK(cudaMemcpyAsync(order, e->f_order.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
+    if (n) CK(cudaMemcpyAsync(route, e->f_route.p, n, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return BB_OK;
+}
+
+int bb_forward_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, const uint32_t* d_miss_idx,
+                            const uint32_t* d_resolve_totals, uint32_t n_cap, uint64_t id_key, uint8_t* d_uq, uint32_t uq_cap,
+                            uint32_t* d_uq_off, uint32_t* d_order, uint32_t* d_group_off, uint8_t* d_route, uint8_t* d_q,
+                            uint32_t q_cap, uint32_t* d_q_off, uint32_t* d_totals, void* stream) {
+    if (!forward_ready(e) || !d_pkts || !d_pkt_off || !d_miss_idx || !d_resolve_totals || !d_uq || !d_uq_off || !d_order ||
+        !d_group_off || !d_route || !d_q || !d_q_off || !d_totals)
+        return BB_ERR_ARG;
+    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
+    int rc = fwd_scratch(e, stream, false, &desc, &fs);
+    if (rc != BB_OK) return rc;
+    return forward_launch(e, desc, fs, d_pkts, d_pkt_off, d_miss_idx, d_resolve_totals, 0, fwd_cap(e, n_cap), id_key, d_uq, uq_cap,
+                          d_uq_off, d_order, d_group_off, d_route, d_q, q_cap, d_q_off, d_totals, (cudaStream_t)stream);
+}
+
+int bb_match_upstreams(bb_engine* e, const uint8_t* resp, const uint32_t* resp_off, const uint32_t* src_ip, const uint16_t* src_port,
+                       uint32_t n_resp, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* route, uint32_t n, uint64_t id_key,
+                       uint8_t* up, uint32_t up_cap, uint32_t* up_off) {
+    if (!forward_ready(e) || !resp_off || !q_off || !up_off || n > fwd_cap(e, bbk::FWD_MAX) || n_resp > BB_MATCH_MAX_RESPONSES)
+        return BB_ERR_ARG;
+    if (n_resp && (!src_ip || !src_port || (resp_off[n_resp] && !resp) || !offsets_ok(resp_off, n_resp))) return BB_ERR_ARG;
+    if (n && (!route || (q_off[n] && !q_pkts) || !offsets_ok(q_off, n))) return BB_ERR_ARG;
+    const uint32_t rbytes = resp_off[n_resp], qbytes = q_off[n];
+    CK(cudaSetDevice(e->device));
+    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
+    int rc;
+    if ((rc = fwd_scratch(e, nullptr, true, &desc, &fs)) || (rc = relay_grow(e->f_resp, (size_t)rbytes + 64)) ||
+        (rc = relay_grow(e->f_respoff, ((size_t)n_resp + 1) * 4)) || (rc = relay_grow(e->f_ip, (size_t)n_resp * 4 + 16)) ||
+        (rc = relay_grow(e->f_port, (size_t)n_resp * 2 + 16)) || (rc = relay_grow(e->f_q, (size_t)qbytes + 64)) ||
+        (rc = relay_grow(e->f_qoff, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->f_route, (size_t)n + 16)) ||
+        (rc = relay_grow(e->f_up, (size_t)rbytes + 64)) || (rc = relay_grow(e->f_upoff, ((size_t)n + 1) * 4)) ||
+        (rc = relay_grow(e->f_tot, 32)))
+        return rc;
+    cudaStream_t st = e->slots[0].stream;
+    if (rbytes) CK(cudaMemcpyAsync(e->f_resp.p, resp, rbytes, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->f_respoff.p, resp_off, ((size_t)n_resp + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (n_resp) CK(cudaMemcpyAsync(e->f_ip.p, src_ip, (size_t)n_resp * 4, cudaMemcpyHostToDevice, st));
+    if (n_resp) CK(cudaMemcpyAsync(e->f_port.p, src_port, (size_t)n_resp * 2, cudaMemcpyHostToDevice, st));
+    if (qbytes) CK(cudaMemcpyAsync(e->f_q.p, q_pkts, qbytes, cudaMemcpyHostToDevice, st));
+    CK(cudaMemcpyAsync(e->f_qoff.p, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
+    if (n) CK(cudaMemcpyAsync(e->f_route.p, route, n, cudaMemcpyHostToDevice, st));
+    // the winners are distinct responses: their bytes fit a buffer of all the responses
+    rc = match_launch(e, desc, fs, (uint8_t*)e->f_resp.p, (uint32_t*)e->f_respoff.p, (uint32_t*)e->f_ip.p, (uint16_t*)e->f_port.p, n_resp,
+                      (uint8_t*)e->f_q.p, (uint32_t*)e->f_qoff.p, (uint8_t*)e->f_route.p, nullptr, n, n, id_key, (uint8_t*)e->f_up.p,
+                      rbytes, (uint32_t*)e->f_upoff.p, (uint32_t*)e->f_tot.p, st);
+    if (rc != BB_OK) return rc;
+    uint32_t tot[4];
+    CK(cudaMemcpyAsync(tot, e->f_tot.p, 16, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    if (tot[0] > up_cap) return BB_ERR_CAPACITY;
+    if (tot[0]) CK(cudaMemcpyAsync(up, e->f_up.p, tot[0], cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(up_off, e->f_upoff.p, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    return BB_OK;
+}
+
+int bb_match_upstreams_device(bb_engine* e, const uint8_t* d_resp, const uint32_t* d_resp_off, const uint32_t* d_src_ip,
+                              const uint16_t* d_src_port, uint32_t n_resp, const uint8_t* d_q, const uint32_t* d_q_off,
+                              const uint8_t* d_route, const uint32_t* d_forward_totals, uint32_t n_cap, uint64_t id_key, uint8_t* d_up,
+                              uint32_t up_cap, uint32_t* d_up_off, uint32_t* d_totals, void* stream) {
+    if (!forward_ready(e) || n_resp > BB_MATCH_MAX_RESPONSES || !d_resp_off || (n_resp && (!d_resp || !d_src_ip || !d_src_port)) ||
+        !d_q || !d_q_off || !d_route || !d_forward_totals || !d_up || !d_up_off || !d_totals)
+        return BB_ERR_ARG;
+    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
+    int rc = fwd_scratch(e, stream, false, &desc, &fs);
+    if (rc != BB_OK) return rc;
+    return match_launch(e, desc, fs, d_resp, d_resp_off, d_src_ip, d_src_port, n_resp, d_q, d_q_off, d_route, d_forward_totals, 0,
+                        fwd_cap(e, n_cap), id_key, d_up, up_cap, d_up_off, d_totals, (cudaStream_t)stream);
 }
 
 int bb_resolve_submit_ex(bb_engine* e, int slot, const uint8_t* pkts, const uint32_t* pkt_off, uint32_t n, uint64_t seed,

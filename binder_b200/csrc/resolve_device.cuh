@@ -383,12 +383,16 @@ __device__ __forceinline__ void size_single(Res& r, uint32_t fixed, uint32_t rr)
 //   domain.indexOf(dnsDomain, domain.length - dnsDomain.length) === -1            -> not ours   (:330-333)
 //   p = domain minus the suffix and the one character before it; dc = p after its last '.';
 //   self.dcs[dc] === undefined (or every upstream of dc is this host)              -> nowhere to ask (:338-343,377-379)
-// Kept out of line: it runs for misses only and must not cost the hit path registers.
-__device__ __noinline__ bool recursion_forwardable(const EngineConst* E, const uint8_t* nm, uint32_t W) {
+// rf_scan() is the scan itself: IDX -> the index of dc in the filter's list or -1 (rf_dc_index(), the forward kernel's
+// route, forward_device.cuh); !IDX -> 1 or 0 (recursion_forwardable(), kept out of line: it runs for misses only and must
+// not cost the hit path registers; this form compiles to the same instructions as the scan written with bool returns).
+template <bool IDX>
+__device__ __forceinline__ int rf_scan(const EngineConst* E, const uint8_t* nm, uint32_t W) {
+    constexpr int NO = IDX ? -1 : 0;
     const uint32_t L = E->rf_dom_len;
-    if (W < 1 + L) return false;                       // name shorter than the suffix
+    if (W < 1 + L) return NO;                          // name shorter than the suffix
     const uint32_t s0 = W - L;                         // wire index where the suffix must start
-    if (s0 < 2) return false;                          // nothing before it: dc = ''
+    if (s0 < 2) return NO;                             // nothing before it: dc = ''
     const uint32_t cw = s0 - 1;                        // the character substring() drops (normally the '.')
     uint32_t nlp = 1u + nm[0], last_b = 0;             // next length byte; last boundary before cw
     bool ok = true;
@@ -400,16 +404,20 @@ __device__ __noinline__ bool recursion_forwardable(const EngineConst* E, const u
             ok &= boundary ? e == '.' : (e != '.' && e == nm[w]);
         }
     }
-    if (!ok) return false;
+    if (!ok) return NO;
     const uint32_t d0 = last_b + 1, dl = cw - d0;      // dc = dotted[d0 .. cw)
-    if (dl == 0 || dl > 63) return false;
+    if (dl == 0 || dl > 63) return NO;
     for (uint32_t k = 0; k < E->rf_ndc; k++) {
         if (E->rf_dc_len[k] != dl) continue;
         bool eq = true;
         for (uint32_t i = 0; i < dl; i++) eq &= E->rf_dc[k][i] == nm[d0 + i];
-        if (eq) return true;
+        if (eq) return IDX ? (int)k : 1;
     }
-    return false;
+    return NO;
+}
+__device__ __forceinline__ int rf_dc_index(const EngineConst* E, const uint8_t* nm, uint32_t W) { return rf_scan<true>(E, nm, W); }
+__device__ __noinline__ bool recursion_forwardable(const EngineConst* E, const uint8_t* nm, uint32_t W) {
+    return rf_scan<false>(E, nm, W) != 0;
 }
 
 // What resolve() does once zk.lookup() has answered (lib/server.js:219-424); shared by the

@@ -219,7 +219,15 @@ struct EngineConst {
     uint8_t  rf_dom[256];        // that domain, dotted
     uint8_t  rf_dc_len[16];
     uint8_t  rf_dc[16][64];      // datacenter names (self.dcs keys), case-sensitive
+    // upstream resolvers of the forward and match kernels (bb_engine_set_recursion_upstreams): what is left of self.dcs
+    // after the own-address filter (lib/recursion.js:205-240,360-379); fu_dc[i] indexes rf_dc
+    uint32_t fu_n;               // entries (0: no table)
+    uint32_t fu_dcmask;          // bit d: datacenter d has at least one upstream
+    uint32_t fu_ip[64];          // IPv4, host byte order (127.0.0.1 = 0x7F000001)
+    uint16_t fu_port[64];
+    uint8_t  fu_dc[64];
 };
+constexpr uint32_t FU_MAX = 64;
 
 // ---- building the per-engine constants (host side; shared by the engine and the CPU emulation harness) ----
 // dotted name -> wire labels without terminator; false if a label is empty or longer than 63 bytes
@@ -263,9 +271,14 @@ inline bool make_engine_const(const char* dns_domain, bool recursion, EngineCons
     for (size_t i = 0; i < n; i++) { const char c = dns_domain[i]; if (!((c >= 'a' && c <= 'z') || (c >= '0' && c <= '9') || c == '_' || c == '-' || c == '.')) C.lean_ok = 0; }
     return true;
 }
+inline void clear_upstreams_const(EngineConst& C) {
+    C.fu_n = 0; C.fu_dcmask = 0;
+    for (uint32_t i = 0; i < 64; i++) { C.fu_ip[i] = 0; C.fu_port[i] = 0; C.fu_dc[i] = 0; }
+}
 // lib/recursion.js:329-344 pre-filter fields (see bb_engine_set_recursion_filter).  false: bad arguments.
+// Setting or removing the filter also clears the upstream table: its datacenter indices refer to the old list.
 inline bool set_recursion_filter_const(EngineConst& C, const char* region_domain, const char* const* dc_names, uint32_t n_dc, bool ptr) {
-    if (!region_domain) { if (C.recursion) C.recursion = 1; return true; }
+    if (!region_domain) { if (C.recursion) C.recursion = 1; clear_upstreams_const(C); return true; }
     if (!C.recursion || n_dc > RF_MAX_DC || (n_dc && !dc_names)) return false;
     size_t L = 0; while (region_domain[L]) ++L;
     if (L > 255) return false;
@@ -280,6 +293,19 @@ inline bool set_recursion_filter_const(EngineConst& C, const char* region_domain
     }
     C.rf_ptr = ptr ? 1 : 0;
     C.recursion = 2;
+    clear_upstreams_const(C);
+    return true;
+}
+// bb_engine_set_recursion_upstreams: false on an engine without recursion, more than FU_MAX entries, or a dc[i] that
+// is not in the filter's list.  n == 0 clears the table.
+inline bool set_recursion_upstreams_const(EngineConst& C, const uint32_t* ip, const uint16_t* port, const uint8_t* dc, uint32_t n) {
+    if (!C.recursion || n > FU_MAX || (n && (!ip || !port || !dc))) return false;
+    for (uint32_t i = 0; i < n; i++) if (C.recursion != 2 || dc[i] >= C.rf_ndc) return false;
+    C.fu_n = n; C.fu_dcmask = 0;
+    for (uint32_t i = 0; i < FU_MAX; i++) {
+        C.fu_ip[i] = i < n ? ip[i] : 0; C.fu_port[i] = i < n ? port[i] : 0; C.fu_dc[i] = i < n ? dc[i] : 0;
+        if (i < n) C.fu_dcmask |= 1u << dc[i];
+    }
     return true;
 }
 

@@ -14,6 +14,14 @@ from . import _lib
 from ._lib import check, lib
 
 ANSWERED, MISS_RECURSE, DROPPED = 0, 1, 2
+ROUTE_PTR, ROUTE_NONE = 16, 17          # forward routes after the 16 datacenter indices (BB_ROUTE_PTR, BB_ROUTE_NONE)
+FORWARD_ROUTES = 18
+
+
+def ip_u32(addr):
+    """Dotted IPv4 -> the host-order integer the forward and match calls take."""
+    a, b, c, d = (int(x) for x in addr.split('.'))
+    return a << 24 | b << 16 | c << 8 | d
 
 
 def repack(out, out_off, out_len):
@@ -183,6 +191,66 @@ class Engine(object):
         """bb_relay_batch_device; pointers are raw device addresses."""
         check(lib().bb_relay_batch_device(self._h, d_q, d_q_off, d_up, d_up_off, n, 1 if tcp else 0, d_out, out_cap, d_out_off,
                                           d_out_len, d_status, d_totals, stream))
+
+    # -- recursion forward and match (bb_forward_batch, bb_match_upstreams, lib/recursion.js:253-280,335-354,382-387) --
+    def set_recursion_upstreams(self, upstreams):
+        """upstreams: [(ipv4 dotted, port, dc index in the filter's list)] (bb_engine_set_recursion_upstreams)."""
+        n = len(upstreams)
+        ip = np.array([ip_u32(a) for a, _, _ in upstreams] or [0], dtype=np.uint32)
+        port = np.array([p for _, p, _ in upstreams] or [0], dtype=np.uint16)
+        dc = np.array([d for _, _, d in upstreams] or [0], dtype=np.uint8)
+        check(lib().bb_engine_set_recursion_upstreams(self._h, ip.ctypes.data, port.ctypes.data, dc.ctypes.data, n))
+
+    def forward_batch(self, data, off, id_key):
+        """Misses data[off[j]:off[j+1]] -> (uq uint8[total], uq_off uint32[n+1], order uint32[n], group_off uint32[19],
+        route uint8[n]): upstream query k = uq[uq_off[k]:uq_off[k+1]] is miss order[k]'s; route r's queries are positions
+        group_off[r] .. group_off[r+1] (16 = PTR, 17 = nowhere to send)."""
+        data = np.ascontiguousarray(data, dtype=np.uint8)
+        off = np.ascontiguousarray(off, dtype=np.uint32)
+        n = len(off) - 1
+        uq = np.empty(max(int(off[n]), 16), dtype=np.uint8)
+        uq_off = np.zeros(n + 1, dtype=np.uint32)
+        order = np.zeros(max(n, 1), dtype=np.uint32)
+        group_off = np.zeros(FORWARD_ROUTES + 1, dtype=np.uint32)
+        route = np.zeros(max(n, 1), dtype=np.uint8)
+        check(lib().bb_forward_batch(self._h, data.ctypes.data, off.ctypes.data, n, id_key & (2 ** 64 - 1), uq.ctypes.data,
+                                     len(uq), uq_off.ctypes.data, order.ctypes.data, group_off.ctypes.data, route.ctypes.data))
+        return uq[:uq_off[n]].copy(), uq_off, order[:n], group_off, route[:n]
+
+    def match_upstreams(self, resp, resp_off, src_ip, src_port, q_data, q_off, route, id_key):
+        """Received datagrams (packed in arrival order, sources as uint32 IPv4 / uint16 port) against a forward call's
+        misses (client queries q_data/q_off and route in miss order) -> (up uint8[total], up_off uint32[n+1]): miss j's
+        accepted upstream response, empty when none."""
+        resp = np.ascontiguousarray(resp, dtype=np.uint8)
+        resp_off = np.ascontiguousarray(resp_off, dtype=np.uint32)
+        src_ip = np.ascontiguousarray(src_ip, dtype=np.uint32)
+        src_port = np.ascontiguousarray(src_port, dtype=np.uint16)
+        q_data = np.ascontiguousarray(q_data, dtype=np.uint8)
+        q_off = np.ascontiguousarray(q_off, dtype=np.uint32)
+        route = np.ascontiguousarray(route, dtype=np.uint8)
+        n_resp, n = len(resp_off) - 1, len(q_off) - 1
+        if len(src_ip) != n_resp or len(src_port) != n_resp or len(route) != n:
+            raise ValueError('one source per response and one route per miss')
+        up = np.empty(max(int(resp_off[n_resp]), 16), dtype=np.uint8)
+        up_off = np.zeros(n + 1, dtype=np.uint32)
+        check(lib().bb_match_upstreams(self._h, resp.ctypes.data, resp_off.ctypes.data, src_ip.ctypes.data, src_port.ctypes.data,
+                                       n_resp, q_data.ctypes.data, q_off.ctypes.data, route.ctypes.data, n,
+                                       id_key & (2 ** 64 - 1), up.ctypes.data, len(up), up_off.ctypes.data))
+        return up[:up_off[n]].copy(), up_off
+
+    def forward_device(self, d_pkts, d_pkt_off, d_miss_idx, d_resolve_totals, n_cap, id_key, d_uq, uq_cap, d_uq_off, d_order,
+                       d_group_off, d_route, d_q, q_cap, d_q_off, d_totals, stream=0):
+        """bb_forward_batch_device; pointers are raw device addresses."""
+        check(lib().bb_forward_batch_device(self._h, d_pkts, d_pkt_off, d_miss_idx, d_resolve_totals, n_cap, id_key & (2 ** 64 - 1),
+                                            d_uq, uq_cap, d_uq_off, d_order, d_group_off, d_route, d_q, q_cap, d_q_off, d_totals,
+                                            stream))
+
+    def match_device(self, d_resp, d_resp_off, d_src_ip, d_src_port, n_resp, d_q, d_q_off, d_route, d_forward_totals, n_cap,
+                     id_key, d_up, up_cap, d_up_off, d_totals, stream=0):
+        """bb_match_upstreams_device; pointers are raw device addresses."""
+        check(lib().bb_match_upstreams_device(self._h, d_resp, d_resp_off, d_src_ip, d_src_port, n_resp, d_q, d_q_off, d_route,
+                                              d_forward_totals, n_cap, id_key & (2 ** 64 - 1), d_up, up_cap, d_up_off, d_totals,
+                                              stream))
 
     # -- device-buffer path (bb_resolve_batch_device); pointers are raw device addresses ------
     def resolve_device(self, d_pkts, d_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status,

@@ -256,6 +256,77 @@ int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t*
                           const uint32_t* d_up_off, uint32_t n, uint32_t flags, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
                           uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_totals, void* stream);
 
+/*
+ * Recursion forward: the upstream queries of a batch of misses, grouped by datacenter, and the matching of the upstream
+ * responses to them.  Replaces Recursion.prototype.resolve's lookup (lib/recursion.js:253-280,335-354,382-387) up to the
+ * point where the replies are built (bb_relay_batch).  DESIGN.md section 14.
+ *
+ * bb_engine_set_recursion_upstreams: the upstream resolvers, what is left of self.dcs after the own-address filter
+ * (:205-240,360-379).  Entry i is ip[i]:port[i] (IPv4 and port in host byte order: 127.0.0.1 = 0x7F000001) of the
+ * datacenter with index dc[i] in the list last passed to bb_engine_set_recursion_filter.  At most 64 entries; n = 0 clears
+ * the table.  Batches already in flight finish on the old table.  BB_ERR_ARG on an engine without `recursion`, without a
+ * filter, or for a dc[i] that is not in the filter.
+ */
+int bb_engine_set_recursion_upstreams(bb_engine* e, const uint32_t* ip, const uint16_t* port, const uint8_t* dc, uint32_t n);
+
+#define BB_FORWARD_MAX 65536            /* misses per forward call: the 16-bit ID space */
+#define BB_ROUTE_PTR 16                 /* route of a PTR miss: every upstream */
+#define BB_ROUTE_NONE 17                /* route of a miss with no upstream to ask (answered REFUSED through the relay) */
+#define BB_MATCH_MAX_RESPONSES 1048576  /* received datagrams per match call */
+/*
+ * bb_forward_batch: miss j = pkts[pkt_off[j] .. pkt_off[j+1]), n <= BB_FORWARD_MAX (and <= max_batch).  For each miss:
+ *   route[j]    the index of its datacenter in the filter's list (the pre-filter's suffix and label scan), BB_ROUTE_PTR
+ *               for a PTR query, BB_ROUTE_NONE when the upstream table has no upstream for it or the packet does not decode
+ *   its upstream query, byte for byte what recursion.py's _exchange sends except the ID: the client's flags & 0x7800
+ *               (opcode kept, RD cleared), QDCOUNT 1, no other records, the client's QNAME, QTYPE and QCLASS; no OPT.
+ *               ID = F(j), a keyed bijection on 16 bits (4-round Feistel network, round keys from id_key): the IDs of
+ *               one call are distinct and cannot be predicted without the key.  Pick a fresh key for every call.
+ * The upstream queries are grouped by route with a stable sort: route r's queries are output positions
+ * group_off[r] .. group_off[r+1] (group_off has BB_ROUTE_NONE + 2 entries), each run in miss order; position k holds
+ * miss order[k], at uq[uq_off[k] .. uq_off[k+1]) (an undecodable packet has an empty query).  A run can be sent to every
+ * upstream of its datacenter with one vector of messages.  BB_ERR_ARG without a filter or an upstream table, for
+ * n > BB_FORWARD_MAX or decreasing offsets; BB_ERR_CAPACITY when the queries do not fit uq_cap.  Synchronous.
+ */
+int bb_forward_batch(bb_engine* e, const uint8_t* pkts, const uint32_t* pkt_off, uint32_t n, uint64_t id_key, uint8_t* uq,
+                     uint32_t uq_cap, uint32_t* uq_off, uint32_t* order, uint32_t* group_off, uint8_t* route);
+/*
+ * Device-resident form of bb_forward_batch, straight from a resolve launch (bb_resolve_batch_device): miss j is packet
+ * d_miss_idx[j] of d_pkts / d_pkt_off, the miss count is d_resolve_totals[1], read on the device (no host round trip
+ * between the launches); n_cap bounds it (the resolve batch's size; more than min(n_cap, BB_FORWARD_MAX) misses is an
+ * error).  Besides the outputs of bb_forward_batch it writes each miss's client query packed in miss order,
+ * d_q[d_q_off[j] .. d_q_off[j+1]): the query input of bb_relay_batch_device and bb_match_upstreams_device.
+ * d_totals[5] = {upstream query bytes, n, error marker, done marker, client query bytes}; the markers equal
+ * bb_engine_launch_epoch() of this call when set (too many misses, or uq_cap / q_cap too small).  Streams as
+ * bb_resolve_batch_device.  Asynchronous.
+ */
+int bb_forward_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, const uint32_t* d_miss_idx,
+                            const uint32_t* d_resolve_totals, uint32_t n_cap, uint64_t id_key, uint8_t* d_uq, uint32_t uq_cap,
+                            uint32_t* d_uq_off, uint32_t* d_order, uint32_t* d_group_off, uint8_t* d_route, uint8_t* d_q,
+                            uint32_t q_cap, uint32_t* d_q_off, uint32_t* d_totals, void* stream);
+/*
+ * bb_match_upstreams: the datagrams received for a forward call, packed in arrival order — response r =
+ * resp[resp_off[r] .. resp_off[r+1]) from src_ip[r]:src_port[r] (host byte order), n_resp <= BB_MATCH_MAX_RESPONSES —
+ * against that call's misses: the client queries q_pkts / q_off and route[] in miss order, n, and its id_key.
+ * Response r is accepted for miss j = F^-1(ID) when j < n, it is at least 12 bytes with QR set, its source is an
+ * upstream of route[j] (any upstream for BB_ROUTE_PTR), QDCOUNT >= 1 and its first question equals the forwarded one
+ * byte for byte (no compression pointer, same case).  The earliest accepted response of each miss wins.  Output: the
+ * winners packed in miss order, up[up_off[j] .. up_off[j+1]), empty for a miss without one — bb_relay_batch's upstream
+ * input as it stands (an empty upstream is a failed lookup: REFUSED, :382-386).  The datagrams are untrusted: every read
+ * is bounds-checked.  BB_ERR_ARG as bb_forward_batch; BB_ERR_CAPACITY when the winners do not fit up_cap.  Synchronous.
+ */
+int bb_match_upstreams(bb_engine* e, const uint8_t* resp, const uint32_t* resp_off, const uint32_t* src_ip, const uint16_t* src_port,
+                       uint32_t n_resp, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* route, uint32_t n, uint64_t id_key,
+                       uint8_t* up, uint32_t up_cap, uint32_t* up_off);
+/*
+ * Device-resident form of bb_match_upstreams: the forward launch's d_q, d_q_off and d_route, its miss count read on the
+ * device from d_forward_totals[1] (bounded by n_cap as in bb_forward_batch_device).  d_totals[4] = {response bytes,
+ * misses answered, overflow marker, done marker}.  Streams as bb_resolve_batch_device.  Asynchronous.
+ */
+int bb_match_upstreams_device(bb_engine* e, const uint8_t* d_resp, const uint32_t* d_resp_off, const uint32_t* d_src_ip,
+                              const uint16_t* d_src_port, uint32_t n_resp, const uint8_t* d_q, const uint32_t* d_q_off,
+                              const uint8_t* d_route, const uint32_t* d_forward_totals, uint32_t n_cap, uint64_t id_key, uint8_t* d_up,
+                              uint32_t up_cap, uint32_t* d_up_off, uint32_t* d_totals, void* stream);
+
 /* Number of kernel launches bb_* calls have issued so far on this engine. */
 uint64_t bb_engine_launch_count(const bb_engine* e);
 /* Epoch (launch number, low 32 bits) of the most recent resolve call on this engine. */
