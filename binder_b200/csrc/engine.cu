@@ -342,12 +342,9 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     }
     const uint32_t my_len = r.rlen;
     const uint32_t my_miss = (qi < nq && r.status == ST_MISS) ? 1u : 0u;
-    // service variant: how many copy jobs this response becomes (its jobs go to the exclusive prefix of these counts)
-    uint32_t my_cnt = 0;
-    if (SVC && my_len && r.ntask) {
-        if (r.ntask >= 2) my_cnt = r.ntask - 2;          // whole answer: the count is a build-time sum
-        else { TaskCount tc = { 0 }; plan_service(P, r, qidx, 0, 0, tc); my_cnt = tc.n; }
-    }
+    // service variant: how many copy jobs this response becomes (its jobs go to the exclusive prefix of these counts);
+    // size_service() counted them while it sized the answer
+    const uint32_t my_cnt = (SVC && my_len && r.ntask) ? r.ntask - 2 : 0u;
 
     STAMP(6);
     // ---- CTA scan of (bytes, misses) ------------------------------------------------------------
@@ -409,7 +406,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     } else if (!overflow && SVC && tile_bytes > (uint32_t)WIN) {
         const uint32_t s_out_a = (uint32_t)__cvta_generic_to_shared(s_out);
         const uint32_t nr = (tile_bytes + WIN - 1) / WIN;                     // <= NROUNDS
-        const uint32_t kr = my_o / WIN;
+        const uint32_t kr = my_len ? my_o / WIN : (uint32_t)NROUNDS;           // the round that writes this thread's response (NROUNDS: none)
         bool jobs = false;
         if (tid < 4) s_opt[tid] = tid == 0 ? 0x04290000u : tid == 1 ? 0x000000B0u : 0u;          // OPT: 00 | 00 29 | 04 B0 | ttl 0 | rdlen 0, zero padded
         if (tid <= NROUNDS) { s_rstart[tid] = 0xFFFFFFFFu; s_tstart[tid] = 0xFFFFFFFFu; }
@@ -443,7 +440,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
             const uint32_t nz = (shift + (x1 - x0) + 15) >> 4;                // pieces are OR-ed into a zeroed buffer
             for (uint32_t i = tid; i < nz; i += T) ((uint4*)s_out)[i] = make_uint4(0, 0, 0, 0);
             __syncthreads();
-            if (my_len && kr == k) {
+            if (kr == k) {
                 WrT<4> w; w.begin(s_out_a, delta + my_o);
                 if (jobs) { emit_head_w(r, w); w.end(); } else emit_fast(P, r, w, qidx);
             }

@@ -75,7 +75,7 @@ struct Res {
     uint32_t status, rk, rcode, tc, opcode, rd, edns, trunc;
     uint32_t owner;          // route mode: rank that owns this query's lookup key
     uint32_t ntask;          // != 0: a service answer that can be assembled from copy jobs (plan_service): header + question by this thread, the
-                             // RRs by anyone.  1: count the jobs by walking the children; 2 + n: it is n jobs (whole answer: build-time sums)
+                             // RRs by anyone.  It is 2 + n for n jobs (size_service counts them)
 };
 
 __device__ __forceinline__ uint32_t lower8(uint32_t c) { return (c - 'A' < 26u) ? c + 32 : c; }
@@ -309,65 +309,90 @@ __device__ __forceinline__ uint32_t dom_owner_len(const Res& r) {
 }
 __device__ __forceinline__ uint32_t dom_wire_len(const Res& r) { return (uint32_t)(r.d_end - r.d_off) + 1; }
 
+// One step of a walk over a service's children in sizing or planning.  Counted only by the host emulation built with
+// -DBB_EMU_WALKS (tests/native/emu_service_jobs.cpp, tools/walk_counts.py).
+#if defined(BB_HOST_EMU) && defined(BB_EMU_WALKS)
+extern thread_local unsigned long long bb_emu_walk_steps;
+#define BB_WALK_STEP() (++bb_emu_walk_steps)
+#else
+#define BB_WALK_STEP() ((void)0)
+#endif
+
+// copy jobs of a piece of `len` bytes (run_tasks copies at most TASK_BYTES per job)
+__device__ __forceinline__ uint32_t piece_jobs(uint32_t len) { return (len + TASK_BYTES - 1) / TASK_BYTES; }
+
 // Sizing of a service answer (lib/server.js:361-416).  When no child is malformed for this query type the
 // sums taken at build time size it from the header alone; the children are walked (in shuffled order) only to
 // find where a malformed child cuts the answer short, or which prefix of the RRs survives truncation.
+// An answer that can be assembled from copy jobs (`jobs_ok`) leaves with its exact job count, r.ntask = 2 + jobs: the
+// same pieces plan_service() makes, counted by the walk that sizes the answer, so that no second walk has to count them.
 __device__ void size_service(const Params& P, Res& r, const SvcView& sv, uint32_t qidx, bool srv, uint32_t fixed) {
     const uint32_t nk = sv.nkids();
     r.nk = nk; r.ntask = 0;
     r.perm = nk <= 16 ? make_perm(nk, P.seed, qidx) : 0;
     const uint32_t dol = dom_owner_len(r), dwl = dom_wire_len(r);
-    uint32_t ans_b = 0, add_b = 0, n_ans = 0, n_add = 0, n_walk = nk;
+    uint32_t ans_b = 0, add_b = 0, n_ans = 0, n_add = 0, n_walk = nk, jobs = 0;
     const uint32_t badbit = srv ? KID_BAD_SRV : KID_BAD_A;
     const bool sums = !(sv.hflags() & (srv ? SVC_BAD_SRV : SVC_BAD_A));
-    if (sums) {
-        if (srv) {
-            n_ans = sv.sum_ports(); ans_b = n_ans * (18 + dwl) + sv.sum_wl_ports();
-            n_add = sv.n_valid(); add_b = sv.sum_wl() + n_add * (dol + 14);
-        } else { n_ans = sv.n_valid(); ans_b = n_ans * (dol + 14); }
-    } else {
-        for (uint32_t t = 0; t < nk; t++) {
-            const uint32_t inf = sv.info(perm_at(r, t, P.seed, qidx)), fl = inf & 0xFF, wl = (inf >> 8) & 0xFF, np = (inf >> 16) & 0xFF;
-            if (fl & badbit) { r.rcode = RC_SERVFAIL; n_walk = t; break; }      // :366-376
-            if (fl & KID_ADDR_NULL) continue;                                    // :378-381
-            if (srv) { ans_b += np * (18 + wl + dwl); n_ans += np; add_b += wl + dol + 14; n_add++; }
-            else { ans_b += dol + 14; n_ans++; }
-        }
-    }
-    r.n_walk = n_walk;
     // The answer is the header, the question and (a prefix of) the children's ready RRs: it can be assembled as
     // independent copy jobs (engine.cu) when the prebuilt owner pointers are this query's — no upper-case letter in its
     // domain part — whether or not it is truncated or cut short by a malformed child.
     const bool jobs_ok = nk <= 16 && r.ptr_tgt == r.d_off;
+    if (sums) {
+        // a whole answer's job count is a build-time sum too (an A answer is one 16-byte RR per child)
+        if (srv) {
+            n_ans = sv.sum_ports(); ans_b = n_ans * (18 + dwl) + sv.sum_wl_ports();
+            n_add = sv.n_valid(); add_b = sv.sum_wl() + n_add * (dol + 14);
+            jobs = sv.jobs_srv();
+        } else { n_ans = sv.n_valid(); ans_b = n_ans * (dol + 14); jobs = n_ans; }
+    } else {
+        for (uint32_t t = 0; t < nk; t++) {
+            BB_WALK_STEP();
+            const uint32_t inf = sv.info(perm_at(r, t, P.seed, qidx)), fl = inf & 0xFF, wl = (inf >> 8) & 0xFF, np = (inf >> 16) & 0xFF;
+            if (fl & badbit) { r.rcode = RC_SERVFAIL; n_walk = t; break; }      // :366-376
+            if (fl & KID_ADDR_NULL) continue;                                    // :378-381
+            if (srv) {
+                const uint32_t a = np * (18 + wl + dwl), d = wl + dol + 14;
+                ans_b += a; n_ans += np; add_b += d; n_add++; jobs += piece_jobs(a) + piece_jobs(d);
+            } else { ans_b += dol + 14; n_ans++; jobs++; }
+        }
+    }
+    r.n_walk = n_walk;
+    const uint32_t opt_job = r.edns ? 1u : 0u;                                  // the OPT is a job of its own
     if (fixed + ans_b + add_b <= r.maxsz) {
         r.keep_ans = n_ans; r.keep_add = n_add; r.rlen = fixed + ans_b + add_b;
-        r.ntask = jobs_ok && (n_ans + n_add) && r.rlen <= (uint32_t)MAXRESP;
-        // a whole answer sized from the build-time sums: its job count is a build-time sum too (an A answer is one
-        // 16-byte RR per child), plus the OPT
-        if (r.ntask && sums) r.ntask = 2 + (srv ? sv.jobs_srv() : n_ans) + (r.edns ? 1u : 0u);
+        if (jobs_ok && (n_ans + n_add) && r.rlen <= (uint32_t)MAXRESP) r.ntask = 2 + jobs + opt_job;
         return;
     }
-    // truncation: keep the longest prefix of [answers..., additionals...] that fits
+    // Truncation: keep the longest prefix of [answers..., additionals...] that fits.  Whether all the answers fit is
+    // known before the walk (fixed + ans_b), so ONE walk finds the cut: inside the answers (no additional survives), or
+    // inside the additionals (an A answer has none, so that is SRV only).  Its job count is the kept answer RRs' —
+    // every child's whole SRV run when the answers fit, which keeps a job-mode walk going past the additionals' cut.
     r.tc = 1;
-    uint32_t total = fixed, ka = 0, kd = 0; bool full = false;
-    for (uint32_t t = 0; t < n_walk && !full; t++) {
+    const bool ans_fit = fixed + ans_b <= r.maxsz;
+    uint32_t total = ans_fit ? fixed + ans_b : fixed, ka = ans_fit ? n_ans : 0, kd = 0;
+    bool add_cut = false;
+    jobs = 0;
+    for (uint32_t t = 0; t < n_walk; t++) {
+        BB_WALK_STEP();
         const uint32_t inf = sv.info(perm_at(r, t, P.seed, qidx)), wl = (inf >> 8) & 0xFF, np = (inf >> 16) & 0xFF;
         if (inf & KID_ADDR_NULL) continue;
         const uint32_t each = srv ? 18 + wl + dwl : dol + 14, cnt = srv ? np : 1;
-        uint32_t take = 0;                                                        // how many of this child's RRs still fit (cnt is 1..3 in practice:
-        while (take < cnt && total + each <= r.maxsz) { total += each; ++take; }  // a compare per RR beats an integer division per child)
-        ka += take;
-        if (take < cnt) full = true;
-    }
-    if (!full && srv) for (uint32_t t = 0; t < n_walk; t++) {
-        const uint32_t inf = sv.info(perm_at(r, t, P.seed, qidx)), wl = (inf >> 8) & 0xFF;
-        if (inf & KID_ADDR_NULL) continue;
-        uint32_t each = wl + dol + 14;
-        if (total + each > r.maxsz) break;
-        total += each; ++kd;
+        if (!ans_fit) {
+            uint32_t take = 0;                                                    // how many of this child's RRs still fit (cnt is 1..3 in practice:
+            while (take < cnt && total + each <= r.maxsz) { total += each; ++take; }   // a compare per RR beats an integer division per child)
+            ka += take; jobs += piece_jobs(take * each);
+            if (take < cnt) break;
+        } else {
+            jobs += piece_jobs(cnt * each);
+            const uint32_t d = wl + dol + 14;
+            if (!add_cut && total + d <= r.maxsz) { total += d; ++kd; jobs += piece_jobs(d); }
+            else if (!jobs_ok) break;
+            else add_cut = true;
+        }
     }
     r.keep_ans = ka; r.keep_add = kd; r.rlen = total;
-    r.ntask = jobs_ok && (ka + kd) && total <= (uint32_t)MAXRESP;
+    if (jobs_ok && (ka + kd) && total <= (uint32_t)MAXRESP) r.ntask = 2 + jobs + opt_job;
 }
 
 // one RR that either fits or is dropped (TC)
@@ -1153,6 +1178,7 @@ __device__ void plan_service(const Params& P, const Res& r, uint32_t qidx, uint3
     uint32_t left = r.keep_ans;
     uint64_t pm = r.perm;                                                     // job mode implies nk <= 16: four bits per position
     for (uint32_t t = 0; t < r.n_walk && left; t++, pm >>= 4) {
+        BB_WALK_STEP();
         const uint32_t k = (uint32_t)pm & 15u, inf = sv.info(k);
         if (inf & KID_ADDR_NULL) continue;
         const uint32_t wl = (inf >> 8) & 0xFF, np = (inf >> 16) & 0xFF;
@@ -1166,6 +1192,7 @@ __device__ void plan_service(const Params& P, const Res& r, uint32_t qidx, uint3
     if (srv) {
         left = r.keep_add; pm = r.perm;
         for (uint32_t t = 0; t < r.n_walk && left; t++, pm >>= 4) {
+            BB_WALK_STEP();
             const uint32_t k = (uint32_t)pm & 15u, inf = sv.info(k);
             if (inf & KID_ADDR_NULL) continue;
             const uint32_t wl = (inf >> 8) & 0xFF;
@@ -1173,10 +1200,10 @@ __device__ void plan_service(const Params& P, const Res& r, uint32_t qidx, uint3
         }
     }
 }
-// a piece becomes ceil(len / TASK_BYTES) jobs
+// a piece becomes ceil(len / TASK_BYTES) jobs (the kernel takes the count from size_service; the tests hold it to this walk)
 struct TaskCount {
     uint32_t n;
-    __device__ void put(uint32_t, uint32_t, uint32_t len, uint32_t, uint32_t) { n += (len + TASK_BYTES - 1) / TASK_BYTES; }
+    __device__ void put(uint32_t, uint32_t, uint32_t len, uint32_t, uint32_t) { n += piece_jobs(len); }
 };
 struct TaskFill {
     Task* tl;
