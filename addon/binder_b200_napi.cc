@@ -391,6 +391,89 @@ static napi_value TcpHubStats(napi_env env, napi_callback_info info) {
     return t;
 }
 
+// A native balancer UDP session (bb_backend_*, include/binder_b200.h):
+//   backendCreate(engine, maxBatch = 16384) -> session
+//   backendFeed(session, bytes: Buffer, seed: BigInt) -> {out: Buffer (frames to write), pkts: Buffer, pktOff: Uint32Array,
+//       srcIp: Uint32Array, srcPort: Uint32Array}   (the misses, for the host's recursion; a failed batch is counted, not thrown)
+//   backendRelay(session, pkts, pktOff, upstream, upOff, dstIp: Uint32Array, dstPort: Uint32Array) -> Buffer (OUTBOUND_UDP
+//       frames of the misses' replies; a failed batch is counted, not thrown)
+//   backendStats(session) -> BigUint64Array(8)   (bb_backend_stat 0..7)
+//   backendDestroy(session)   (also done when the session is garbage-collected)
+struct BackendRef { bb_backend* b; };
+static bb_backend* BackendOf(napi_env env, napi_value v) {
+    void* p = nullptr;
+    if (napi_get_value_external(env, v, &p) != napi_ok || !p) return nullptr;
+    return ((BackendRef*)p)->b;
+}
+static napi_value BackendCreate(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* e; NAPI_OK(napi_get_value_external(env, argv[0], &e));
+    uint32_t maxb = 1u << 14; if (argc > 1) napi_get_value_uint32(env, argv[1], &maxb);
+    int err = 0;
+    bb_backend* b = bb_backend_create((bb_engine*)e, maxb, &err);
+    if (!b) return Throw(env, err);
+    napi_value ext;
+    NAPI_OK(napi_create_external(env, new BackendRef{b}, [](napi_env, void* p, void*) {
+        bb_backend_destroy(((BackendRef*)p)->b); delete (BackendRef*)p; }, nullptr, &ext));
+    return ext;
+}
+static napi_value BackendFeed(napi_env env, napi_callback_info info) {
+    size_t argc = 3; napi_value argv[3];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    bb_backend* b = BackendOf(env, argv[0]); if (!b) return Throw(env, BB_ERR_ARG);
+    void* data; size_t len; NAPI_OK(napi_get_buffer_info(env, argv[1], &data, &len));
+    uint64_t seed = 0; bool lossless; napi_get_value_bigint_uint64(env, argv[2], &seed, &lossless);
+    const uint8_t* out = nullptr; size_t out_len = 0; bb_backend_misses m; memset(&m, 0, sizeof m);
+    int rc = bb_backend_feed(b, (const uint8_t*)data, len, seed, &out, &out_len, &m);
+    if (rc == BB_ERR_ARG) return Throw(env, rc);
+    napi_value res; NAPI_OK(napi_create_object(env, &res));
+    const uint32_t zero = 0;
+    napi_set_named_property(env, res, "out", CopyBuffer(env, out, out_len));
+    napi_set_named_property(env, res, "pkts", CopyBuffer(env, m.pkts, m.n ? m.pkt_off[m.n] : 0));
+    napi_set_named_property(env, res, "pktOff", U32Array(env, m.n ? m.pkt_off : &zero, (size_t)m.n + 1));
+    napi_set_named_property(env, res, "srcIp", U32Array(env, m.src_ip, m.n));
+    napi_set_named_property(env, res, "srcPort", U32Array(env, m.src_port, m.n));
+    return res;
+}
+static bool U32Of(napi_env env, napi_value v, size_t n, const uint32_t** p) {
+    napi_typedarray_type tt; size_t len; void* d; napi_value ab; size_t bo;
+    if (napi_get_typedarray_info(env, v, &tt, &len, &d, &ab, &bo) != napi_ok || tt != napi_uint32_array || len != n) return false;
+    *p = (const uint32_t*)d;
+    return true;
+}
+static napi_value BackendRelay(napi_env env, napi_callback_info info) {
+    size_t argc = 7; napi_value argv[7];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    bb_backend* b = BackendOf(env, argv[0]); if (!b) return Throw(env, BB_ERR_ARG);
+    void* pk; size_t pklen; NAPI_OK(napi_get_buffer_info(env, argv[1], &pk, &pklen));
+    void* up; size_t uplen; NAPI_OK(napi_get_buffer_info(env, argv[3], &up, &uplen));
+    const uint32_t *qo, *uo, *ip, *port; size_t qn, un;
+    if (!check_off(env, argv[2], pklen, &qo, &qn) || !check_off(env, argv[4], uplen, &uo, &un) || qn != un ||
+        !U32Of(env, argv[5], qn - 1, &ip) || !U32Of(env, argv[6], qn - 1, &port)) return Throw(env, BB_ERR_ARG);
+    const uint8_t* out = nullptr; size_t out_len = 0;
+    int rc = bb_backend_relay(b, (const uint8_t*)pk, qo, (const uint8_t*)up, uo, ip, port, (uint32_t)(qn - 1), &out, &out_len);
+    if (rc == BB_ERR_ARG) return Throw(env, rc);              // a failed batch is counted (backendStats), not thrown
+    return CopyBuffer(env, out, out_len);
+}
+static napi_value BackendStats(napi_env env, napi_callback_info info) {
+    size_t argc = 1; napi_value argv[1];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    bb_backend* b = BackendOf(env, argv[0]); if (!b) return Throw(env, BB_ERR_ARG);
+    void* p; napi_value ab, t;
+    NAPI_OK(napi_create_arraybuffer(env, 8 * 8, &p, &ab)); NAPI_OK(napi_create_typedarray(env, napi_biguint64_array, 8, ab, 0, &t));
+    for (int i = 0; i < 8; i++) ((uint64_t*)p)[i] = bb_backend_stat(b, i);
+    return t;
+}
+static napi_value BackendDestroy(napi_env env, napi_callback_info info) {
+    size_t argc = 1; napi_value argv[1];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* p; NAPI_OK(napi_get_value_external(env, argv[0], &p));
+    bb_backend_destroy(((BackendRef*)p)->b);
+    ((BackendRef*)p)->b = nullptr;                            // the finalizer then frees only the reference
+    return nullptr;
+}
+
 static napi_value Init(napi_env env, napi_value exports) {
     napi_property_descriptor d[] = {
         { "zoneBuild", nullptr, ZoneBuild, nullptr, nullptr, nullptr, napi_default, nullptr },
@@ -414,6 +497,11 @@ static napi_value Init(napi_env env, napi_value exports) {
         { "tcpHubClose", nullptr, TcpHubClose, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "tcpHubRelay", nullptr, TcpHubRelay, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "tcpHubStats", nullptr, TcpHubStats, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "backendCreate", nullptr, BackendCreate, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "backendFeed", nullptr, BackendFeed, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "backendRelay", nullptr, BackendRelay, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "backendStats", nullptr, BackendStats, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "backendDestroy", nullptr, BackendDestroy, nullptr, nullptr, nullptr, napi_default, nullptr },
     };
     napi_define_properties(env, exports, sizeof d / sizeof d[0], d);
     return exports;

@@ -87,6 +87,7 @@ SYMBOLS = {
     'bb_backend_create': (_c.c_void_p, [_c.c_void_p, _c.c_uint32, _c.POINTER(_c.c_int)]),
     'bb_backend_destroy': (None, [_c.c_void_p]),
     'bb_backend_feed': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_uint64, _c.c_void_p, _c.c_void_p, _c.c_void_p]),
+    'bb_backend_relay': (_c.c_int, [_c.c_void_p] * 7 + [_c.c_uint32, _c.c_void_p, _c.c_void_p]),
     'bb_backend_stat': (_c.c_uint64, [_c.c_void_p, _c.c_int]),
     'bb_tcp_hub_create': (_c.c_void_p, [_c.c_void_p, _c.c_uint32, _c.POINTER(_c.c_int)]),
     'bb_tcp_hub_destroy': (None, [_c.c_void_p]),

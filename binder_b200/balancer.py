@@ -18,11 +18,16 @@ session that opens with INBOUND_TCP {3, source IPv4, source port} (12 bytes), is
 then carries the client's raw 2-byte length-prefixed DNS stream both ways (backend.c:60-75, tcp_proxy.c:160-300).
 TcpHub / NativeTcpHub hold many such sessions and resolve the messages that complete on all of them as one TCP batch.
 A host routes a new AF_UNIX connection by its first frame: CLIENT_HELLO to a Backend, INBOUND_TCP to the hub.
+
+Misses (lib/server.js:110-113,222-225) go to the recursion with the owner's sink (recursion.submit): a Backend submits
+its own with the source address as the tag and relays what its sink drains into OUTBOUND_UDP frames (relay(), UDP size
+limits); a hub's host submits flush()'s misses with the session id as the tag and hands what it drains to hub.relay().
 """
 import struct
 
 import numpy as np
 
+from .recursion import QueueSink, split_packets
 from .server import TcpFramer, pack_packets
 
 CLIENT_HELLO, INBOUND_UDP, INBOUND_TCP, CLIENT_HEARTBEAT = 1, 2, 3, 4
@@ -94,12 +99,21 @@ def build_frames(out, out_off, out_len, status, dst_ip, dst_port, control=()):
 
 
 class Backend(object):
-    """One balancer session: feed() bytes read from the AF_UNIX socket, get bytes to write back."""
+    """One balancer session: feed() bytes read from the AF_UNIX socket, get bytes to write back.
 
-    def __init__(self, resolver, recursion=None, shuffle_seed=1):
+    With a recursion, feed() submits every miss with this session's sink (a QueueSink that calls `wake`, from the
+    recursion thread, when a window arrives) and the source (ip, port) as the tag; drain() then returns the OUTBOUND_UDP
+    frames of the relays that arrived.  relay(queries, upstreams, dst) builds them on `relayer` (anything with
+    relay_batch; the resolver by default) in batches of max_batch, as NativeBackend.relay (bb_backend_relay) does: a
+    failed batch gets no frames and is counted."""
+
+    def __init__(self, resolver, recursion=None, shuffle_seed=1, relayer=None, max_batch=1 << 14, wake=None):
         self.resolver, self.recursion, self.seed = resolver, recursion, shuffle_seed
+        self.relayer = relayer if relayer is not None else resolver
+        self.max_batch = max_batch
+        self.sink = QueueSink(wake)
         self.pending = b''
-        self.counters = {'udp': 0, 'answered': 0, 'missed': 0, 'dropped': 0}
+        self.counters = {'udp': 0, 'answered': 0, 'missed': 0, 'dropped': 0, 'relayed': 0, 'relay_failed': 0}
 
     def feed(self, chunk):
         self.pending += bytes(chunk)
@@ -115,8 +129,27 @@ class Backend(object):
         if self.recursion is not None:
             for i in miss:
                 i = int(i)
-                self.recursion.resolve(bytes(data[off[i]:off[i + 1]]), (int(ips[i]), int(ports[i])))
+                self.recursion.submit(bytes(data[off[i]:off[i + 1]]), self.sink, (int(ips[i]), int(ports[i])))
         return build_frames(out, out_off, out_len, status, ips, ports, control)
+
+    def relay(self, queries, upstreams, dst):
+        """Replies to misses (query i answered from upstream response i, b'' = the lookup failed) -> bytes of one
+        OUTBOUND_UDP frame per answered reply, addressed to dst[i] = (ip, port)."""
+        c, frames = self.counters, []
+        for k0 in range(0, len(queries), self.max_batch):
+            qs, us, ds = queries[k0:k0 + self.max_batch], upstreams[k0:k0 + self.max_batch], dst[k0:k0 + self.max_batch]
+            try:
+                out, out_off, out_len, status = self.relayer.relay_batch(*(pack_packets(qs) + pack_packets(us)))
+            except Exception:                        # BinderError (capacity, CUDA): this batch gets no frames
+                c['relay_failed'] += len(qs)
+                continue
+            c['relayed'] += int((np.asarray(status) == 0).sum())
+            frames.append(build_frames(out, out_off, out_len, status, [ip for ip, _ in ds], [p for _, p in ds]))
+        return b''.join(frames)
+
+    def drain(self):
+        """Bytes of the OUTBOUND_UDP frames for the relays the recursion delivered since the last call."""
+        return b''.join(self.relay(split_packets(q, qo), split_packets(u, uo), tags) for q, qo, u, uo, tags in self.sink.drain())
 
 
 # ---- the same protocol, natively (csrc/balancer_frames.cpp) ---------------------------------------------
@@ -157,40 +190,58 @@ def build_frames_native(out, out_off, out_len, status, dst_ip, dst_port, control
 class NativeBackend(object):
     """bb_backend: one balancer session in the C library (frames in -> bb_resolve_batch -> frames out)."""
 
-    def __init__(self, engine, max_batch=1 << 14):
+    def __init__(self, engine, max_batch=1 << 14, lib=None):
         import ctypes
-        from ._lib import BinderError, lib
+        from ._lib import BinderError, lib as _lib
+        self._L = lib if lib is not None else _lib()
         err = ctypes.c_int(0)
-        self._h = lib().bb_backend_create(engine._h, max_batch, ctypes.byref(err))
+        self._h = self._L.bb_backend_create(engine._h, max_batch, ctypes.byref(err))
         if not self._h:
             raise BinderError(err.value)
-        self._engine = engine
+        self._engine, self.last_rc = engine, 0
 
     def feed(self, chunk, seed):
         """-> (bytes to write back, [(packet, src_ip, src_port)] handed to recursion)"""
         import ctypes
-        from ._lib import check, lib
+        from ._lib import check
 
         class Misses(ctypes.Structure):
             _fields_ = [('n', ctypes.c_uint32), ('pkts', ctypes.POINTER(ctypes.c_uint8)), ('pkt_off', ctypes.POINTER(ctypes.c_uint32)),
                         ('src_ip', ctypes.POINTER(ctypes.c_uint32)), ('src_port', ctypes.POINTER(ctypes.c_uint32))]
         chunk = bytes(chunk)
         out, out_len, m = ctypes.POINTER(ctypes.c_uint8)(), ctypes.c_size_t(0), Misses()
-        check(lib().bb_backend_feed(self._h, chunk, len(chunk), seed, ctypes.byref(out), ctypes.byref(out_len), ctypes.byref(m)))
+        check(self._L.bb_backend_feed(self._h, chunk, len(chunk), seed, ctypes.byref(out), ctypes.byref(out_len), ctypes.byref(m)))
         data = ctypes.string_at(out, out_len.value) if out_len.value else b''
         misses = [(ctypes.string_at(ctypes.addressof(m.pkts.contents) + m.pkt_off[i], m.pkt_off[i + 1] - m.pkt_off[i]),
                    int(m.src_ip[i]), int(m.src_port[i])) for i in range(m.n)]
         return data, misses
 
+    def relay(self, queries, upstreams, dst):
+        """bb_backend_relay: the same frames as Backend.relay.  A failed batch is counted (stats()['relay_failed']), not
+        raised: its code is in last_rc."""
+        import ctypes
+        from ._lib import check
+        if not self._h:
+            check(-1)
+        (qd, qo), (ud, uo) = pack_packets(queries), pack_packets(upstreams)
+        ip = np.ascontiguousarray([a for a, _ in dst], dtype=np.uint32)
+        port = np.ascontiguousarray([p for _, p in dst], dtype=np.uint32)
+        out, out_len = ctypes.POINTER(ctypes.c_uint8)(), ctypes.c_size_t(0)
+        rc = self._L.bb_backend_relay(self._h, qd.ctypes.data, qo.ctypes.data, ud.ctypes.data, uo.ctypes.data,
+                                      ip.ctypes.data if ip.size else None, port.ctypes.data if port.size else None, len(ip),
+                                      ctypes.byref(out), ctypes.byref(out_len))
+        if rc == -1:
+            check(rc)
+        self.last_rc = rc
+        return ctypes.string_at(out, out_len.value) if out_len.value else b''
+
     def stats(self):
-        from ._lib import lib
-        keys = ('udp', 'answered', 'missed', 'dropped', 'pending_bytes')
-        return {k: int(lib().bb_backend_stat(self._h, i)) for i, k in enumerate(keys)}
+        keys = ('udp', 'answered', 'missed', 'dropped', 'pending_bytes', 'failed', 'relayed', 'relay_failed')
+        return {k: int(self._L.bb_backend_stat(self._h, i)) for i, k in enumerate(keys)}
 
     def close(self):
-        from ._lib import lib
         if getattr(self, '_h', None):
-            lib().bb_backend_destroy(self._h)
+            self._L.bb_backend_destroy(self._h)
             self._h = None
 
     def __del__(self):

@@ -8,11 +8,11 @@
 // which is already "batched raw packets + source address".  bb_frames_parse turns a byte stream into the
 // engine's batch container, bb_frames_build turns results back into frames, and bb_backend is a session that
 // does both around bb_resolve_batch, so a native backend can sit on the socket where a Node backend
-// (lib/server.js:621-631 -> mname) sits today.  Host code only: no CUDA in this file.
-#include "../../include/binder_b200.h"
+// (lib/server.js:621-631 -> mname) sits today (its relays, bb_backend_relay: balancer_relay.cpp).  Host code only: no
+// CUDA in this file.
+#include "balancer_backend.h"
 
 #include <cstring>
-#include <vector>
 
 namespace {
 inline uint32_t rd32(const uint8_t* p) { return (uint32_t)p[0] | (uint32_t)p[1] << 8 | (uint32_t)p[2] << 16 | (uint32_t)p[3] << 24; }
@@ -74,20 +74,7 @@ int bb_frames_build(const uint8_t* resp, const uint32_t* resp_off, const uint16_
 
 }  // extern "C"
 
-// ---- one balancer session around an engine ----------------------------------------------------------
-struct bb_backend {
-    bb_engine* e = nullptr; uint32_t max_batch = 0, max_bytes = 0;
-    std::vector<uint8_t> pending;                      // bytes of an incomplete trailing frame
-    // batch containers (pinned: the engine then writes results straight into them)
-    uint8_t* pkts = nullptr; uint32_t* pkt_off = nullptr; uint32_t* ip = nullptr; uint32_t* port = nullptr;
-    uint8_t* resp = nullptr; uint32_t resp_cap = 0; uint32_t* resp_off = nullptr; uint16_t* resp_len = nullptr;
-    uint8_t* status = nullptr; uint32_t* miss = nullptr;
-    std::vector<uint8_t> out;                          // frames to write back
-    std::vector<uint8_t> m_pkts; std::vector<uint32_t> m_off, m_ip, m_port;    // handed-off misses of the last feed
-    uint64_t n_udp = 0, n_answered = 0, n_missed = 0, n_dropped = 0, n_failed = 0;
-    uint32_t qidx_next = 0;                             // query index of the next batch's first query within the current feed (keys the shuffle)
-};
-
+// ---- one balancer session around an engine (struct bb_backend: balancer_backend.h) -------------------
 extern "C" {
 
 bb_backend* bb_backend_create(bb_engine* e, uint32_t max_batch, int* err) {
@@ -174,7 +161,8 @@ int bb_backend_feed(bb_backend* b, const uint8_t* in, size_t in_len, uint64_t sh
 
 uint64_t bb_backend_stat(const bb_backend* b, int what) {
     if (!b) return 0;
-    switch (what) { case 0: return b->n_udp; case 1: return b->n_answered; case 2: return b->n_missed; case 3: return b->n_dropped; case 4: return b->pending.size(); case 5: return b->n_failed; }
+    switch (what) { case 0: return b->n_udp; case 1: return b->n_answered; case 2: return b->n_missed; case 3: return b->n_dropped; case 4: return b->pending.size(); case 5: return b->n_failed;
+                    case 6: return b->n_relayed; case 7: return b->n_relay_failed; }
     return 0;
 }
 

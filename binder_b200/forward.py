@@ -1,13 +1,13 @@
 """GpuRecursion: binder's Recursion (lib/recursion.js:253-388) for binder_b200/server.py with the upstream exchange on the
-GPU.  Same interface as binder_b200.recursion.Recursion — resolve(packet, addr, sock) for every miss, close() — so
-Server takes it through options['recursion'] unchanged.
+GPU.  Same interface as binder_b200.recursion.Recursion — resolve(packet, addr, sock) for a UDP miss, submit(packet,
+sink, tag) for a miss of another transport owner, close() — so Server takes it through options['recursion'] unchanged.
 
-Per collection window: bb_forward_batch builds every miss's upstream query (keyed IDs, RD cleared, no OPT) and groups
-them by datacenter; the host sends each datacenter's run to each of its upstreams from one fresh socket; it receives
-until every forwarded miss has an accepted response or the 3 s of lib/recursion.js:257 have passed, bb_match_upstreams
-picks each miss's response, and bb_relay_batch builds the replies, which go out from the listener's socket.  The host
-reads no byte of a query or a response: its per-miss work is the socket calls.  TCP misses are not answered here, as in
-Recursion.
+Per collection window, the exchange (transport-blind): bb_forward_batch builds every miss's upstream query (keyed IDs,
+RD cleared, no OPT) and groups them by datacenter; the host sends each datacenter's run to each of its upstreams from
+one fresh socket; it receives until every forwarded miss has an accepted response or the 3 s of lib/recursion.js:257
+have passed, and bb_match_upstreams picks each miss's response.  Then the delivery (recursion.deliver): the UDP misses'
+replies are built by one bb_relay_batch and go out from the listener's socket; every other sink gets its misses and
+their upstream responses once.  The host reads no byte of a query or a response: its per-miss work is the socket calls.
 """
 import os
 import queue
@@ -19,6 +19,7 @@ import time
 import numpy as np
 
 from .engine import FORWARD_ROUTES, ROUTE_PTR, ip_u32
+from .recursion import UdpSink, deliver
 from .server import pack_packets
 
 FORWARD_MAX = 65536
@@ -49,7 +50,9 @@ class GpuRecursion(object):
         resolver.set_recursion_upstreams(table)
         self.timeout = timeout
         self.window_s = window_s
-        self.counters = {'relayed': 0, 'forwarded': 0, 'upstream_answers': 0, 'tcp_skipped': 0, 'failed_batches': 0}
+        self.counters = {'relayed': 0, 'forwarded': 0, 'upstream_answers': 0, 'tcp_skipped': 0, 'failed_batches': 0,
+                         'delivered': 0}
+        self._udp = UdpSink(resolver, self.counters)
         self._q = queue.Queue()
         self._stop = threading.Event()
         self._thread = threading.Thread(target=self._loop, daemon=True)
@@ -60,7 +63,11 @@ class GpuRecursion(object):
         if addr is None:
             self.counters['tcp_skipped'] += 1
             return
-        self._q.put((bytes(packet), addr, sock))
+        self._q.put((bytes(packet), self._udp, (addr, sock)))
+
+    def submit(self, packet, sink, tag):
+        """One miss of a transport owner: its upstream response comes back through sink.relay(..., tags) with `tag`."""
+        self._q.put((bytes(packet), sink, tag))
 
     def close(self):
         self._stop.set()
@@ -136,12 +143,13 @@ class GpuRecursion(object):
 
     def _relay(self, batch):
         q_data, q_off = pack_packets([p for p, _, _ in batch])
-        up, up_off = self._exchange(q_data, q_off)
-        out, out_off, out_len, status = self.resolver.relay_batch(q_data, q_off, up, up_off)
-        for i, (_, addr, sock) in enumerate(batch):
-            if status[i] == 0:
-                try:
-                    sock.sendto(out[out_off[i]:out_off[i] + out_len[i]].tobytes(), addr)
-                    self.counters['relayed'] += 1
-                except OSError:
-                    pass
+        try:
+            up, up_off = self._exchange(q_data, q_off)
+        except Exception:                 # BinderError (capacity, CUDA): the UDP misses get no replies; the other owners
+            self.counters['failed_batches'] += 1      # get failed lookups (REFUSED), so what they owe is settled
+            batch = [m for m in batch if m[1] is not self._udp]
+            if not batch:
+                return
+            q_data, q_off = pack_packets([p for p, _, _ in batch])
+            up, up_off = pack_packets([b''] * len(batch))
+        deliver(batch, q_data, q_off, up, up_off, self.counters)

@@ -2,11 +2,19 @@
 is forwarded to an upstream resolver of its datacenter, and the upstream's response becomes binder's reply on the GPU
 (`resolver.relay_batch`, bb_relay_batch: lib/recursion.js:287-327 as a kernel).  Nothing here encodes a DNS answer.
 
-It plugs into Server through options['recursion'], whose resolve(packet, addr, sock) the listener calls for every miss.
-UDP misses are answered: the misses of one collection window are forwarded together, their upstream responses (or
-nothing, after the 3 s timeout of lib/recursion.js:257) are relayed as ONE batch, and each reply is sent from `sock` to
-`addr`.  TCP misses (addr None, on a socket the TCP loop owns) are not answered by this helper; a host that wants them
-calls relay_batch(..., tcp=True) itself (Engine.relay_batch, bb_relay_batch with BB_BATCH_TCP).
+It plugs into Server through options['recursion'].  The misses of one collection window, from every transport, are
+forwarded together (the exchange); their upstream responses (or nothing, after the 3 s timeout of lib/recursion.js:257)
+are then delivered per transport owner (the delivery):
+  - resolve(packet, addr, sock): a UDP miss of a listener this object may send from.  The window's UDP misses are relayed
+    as ONE batch and each reply is sent from `sock` to `addr`.  resolve(packet, None, sock) is a TCP miss of a caller that
+    has not moved to submit(): it is counted in tcp_skipped and not answered.
+  - submit(packet, sink, tag): a miss of a transport owner (the TCP loop, a balancer session, a TCP hub).  After the
+    exchange each sink with misses in the window is called once, sink.relay(q_data, q_off, up, up_off, tags), with its
+    misses in miss order; up[up_off[i]:up_off[i+1]] is miss i's upstream response, empty when the lookup failed.  A sink
+    belongs to an owner, not to a connection or a session: the tag tells the owner's connections apart, so a window costs
+    at most one relay launch per owner.
+Sinks run on the recursion thread.  QueueSink hands a window to a single-threaded owner, which relays it with its own
+engine (relay_batch, tcp=True over TCP) and frames the replies for its transport.
 """
 import os
 import queue
@@ -37,6 +45,72 @@ def _question(pkt):
     return wire, qtype, qclass, '.'.join(labels)
 
 
+def split_packets(data, off):
+    """(packed data, offsets[n+1]) -> [bytes]"""
+    return [bytes(data[int(off[i]):int(off[i + 1])]) for i in range(len(off) - 1)]
+
+
+class QueueSink(object):
+    """The sink of a single-threaded transport owner.  relay() runs on the recursion thread: it queues the window's
+    (q_data, q_off, up, up_off, tags) and calls wake(); the owner calls drain() on its own thread."""
+
+    def __init__(self, wake=None):
+        self._lock = threading.Lock()
+        self._items = []
+        self._wake = wake
+
+    def relay(self, q_data, q_off, up, up_off, tags):
+        with self._lock:
+            self._items.append((q_data, q_off, up, up_off, list(tags)))
+        if self._wake is not None:
+            self._wake()
+
+    def drain(self):
+        """-> [(q_data, q_off, up, up_off, tags)] queued since the last drain, oldest first"""
+        with self._lock:
+            items, self._items = self._items, []
+        return items
+
+
+class UdpSink(object):
+    """resolve()'s delivery: the window's UDP misses relayed as one batch on `resolver`, each reply sent from the
+    listener's socket to the client; the tag is (addr, sock).  A failed relay batch gets no replies and is counted."""
+
+    def __init__(self, resolver, counters):
+        self.resolver, self.counters = resolver, counters
+
+    def relay(self, q_data, q_off, up, up_off, tags):
+        try:
+            out, out_off, out_len, status = self.resolver.relay_batch(q_data, q_off, up, up_off)
+        except Exception:                 # BinderError (capacity, CUDA): this window gets no replies
+            self.counters['failed_batches'] += 1
+            return
+        for i, (addr, sock) in enumerate(tags):
+            if status[i] == 0:
+                try:
+                    sock.sendto(out[out_off[i]:out_off[i] + out_len[i]].tobytes(), addr)
+                    self.counters['relayed'] += 1
+                except OSError:
+                    pass
+
+
+def deliver(batch, q_data, q_off, up, up_off, counters):
+    """The delivery of one window: batch[i] = (packet, sink, tag), (q_data, q_off) its packets and (up, up_off) their
+    upstream responses, packed in batch order.  Each sink is called once, with its own misses in batch order."""
+    groups = {}
+    for i, (_, sink, _) in enumerate(batch):
+        groups.setdefault(id(sink), (sink, []))[1].append(i)
+    for sink, idx in groups.values():
+        if len(idx) == len(batch):
+            q, qo, u, uo = q_data, q_off, up, up_off
+        else:
+            q, qo = pack_packets([bytes(q_data[int(q_off[i]):int(q_off[i + 1])]) for i in idx])
+            u, uo = pack_packets([bytes(up[int(up_off[i]):int(up_off[i + 1])]) for i in idx])
+        if not isinstance(sink, UdpSink):
+            counters['delivered'] += len(idx)
+        sink.relay(q, qo, u, uo, [batch[i][2] for i in idx])
+
+
 class Recursion(object):
     """resolver   an Engine created with recursion=True that this object uses alone (or anything with the same
                   relay_batch, such as the CPU oracle in the tests)
@@ -51,7 +125,9 @@ class Recursion(object):
         self.my_addrs = set(my_addrs)
         self.timeout = timeout
         self.window_s = window_s
-        self.counters = {'relayed': 0, 'forwarded': 0, 'upstream_answers': 0, 'tcp_skipped': 0, 'failed_batches': 0}
+        self.counters = {'relayed': 0, 'forwarded': 0, 'upstream_answers': 0, 'tcp_skipped': 0, 'failed_batches': 0,
+                         'delivered': 0}
+        self._udp = UdpSink(resolver, self.counters)
         self._q = queue.Queue()
         self._stop = threading.Event()
         self._thread = threading.Thread(target=self._loop, daemon=True)
@@ -74,7 +150,11 @@ class Recursion(object):
         if addr is None:
             self.counters['tcp_skipped'] += 1
             return
-        self._q.put((bytes(packet), addr, sock))
+        self._q.put((bytes(packet), self._udp, (addr, sock)))
+
+    def submit(self, packet, sink, tag):
+        """One miss of a transport owner: its reply comes back through sink.relay(..., tags) with `tag`."""
+        self._q.put((bytes(packet), sink, tag))
 
     def close(self):
         self._stop.set()
@@ -148,15 +228,4 @@ class Recursion(object):
         ups = self._exchange(batch)
         q_data, q_off = pack_packets([p for p, _, _ in batch])
         u_data, u_off = pack_packets(ups)
-        try:
-            out, out_off, out_len, status = self.resolver.relay_batch(q_data, q_off, u_data, u_off)
-        except Exception:                 # BinderError (capacity, CUDA): this window gets no replies
-            self.counters['failed_batches'] += 1
-            return
-        for i, (_, addr, sock) in enumerate(batch):
-            if status[i] == 0:
-                try:
-                    sock.sendto(out[out_off[i]:out_off[i] + out_len[i]].tobytes(), addr)
-                    self.counters['relayed'] += 1
-                except OSError:
-                    pass
+        deliver(batch, q_data, q_off, u_data, u_off, self.counters)

@@ -10,7 +10,12 @@ TCP (mname's listenTcp, lib/server.js:643-652): every connection is a stream of 
 by its length as two big-endian bytes (RFC 1035 4.2.2; deps/mname-balancer/tcp_proxy.c:10-26 relays the
 same framing).  TcpFramer reassembles them; messages from all connections that complete inside one
 aggregation window form ONE batch, resolved with tcp=True (no UDP size limit), and each response goes
-back on its connection with its own length prefix, in arrival order per connection.
+back on its connection with its own length prefix, in arrival order per connection.  A TCP miss is submitted to the
+recursion (recursion.submit) with the TCP loop's queue sink, the connection as its tag, when the recursion has submit()
+and the resolver has relay_batch(); the loop relays each window it drains with tcp=True and appends every reply to its
+connection, length-prefixed.  Relayed replies may overtake local answers on the same connection (RFC 7766 allows it: the
+ID matches them).  A connection owed a relay stays open through the idle sweep and after a half-close until the reply
+is written.
 
 The resolver is injected, so the CPU-only plumbing test (BASELINE config 1) drives this same code
 with the CPU oracle, while production passes an Engine.
@@ -64,11 +69,12 @@ def pack_packets(pkts):
 
 
 class TcpConn(object):
-    """One TCP connection: reassembly state, bytes still to send, queries it is owed answers for."""
-    __slots__ = ('framer', 'outq', 'waiting', 'eof', 'last')
+    """One TCP connection: reassembly state, bytes still to send, queries it is owed answers (or relays) for, and
+    whether it is registered with the selector (a half-closed connection that only waits for a relay is not)."""
+    __slots__ = ('framer', 'outq', 'waiting', 'eof', 'last', 'reg')
 
     def __init__(self, now):
-        self.framer, self.outq, self.waiting, self.eof, self.last = TcpFramer(), bytearray(), 0, False, now
+        self.framer, self.outq, self.waiting, self.eof, self.last, self.reg = TcpFramer(), bytearray(), 0, False, now, True
 
 
 class Server(object):
@@ -84,7 +90,8 @@ class Server(object):
         self.max_batch = options.get('max_batch', 4096)
         self.recursion = options.get('recursion')
         self.counters = {'queries': 0, 'answered': 0, 'missed': 0, 'dropped': 0, 'batches': 0,
-                         'tcp_queries': 0, 'tcp_batches': 0, 'tcp_connections': 0, 'tcp_refused': 0, 'failed_batches': 0}
+                         'tcp_queries': 0, 'tcp_batches': 0, 'tcp_connections': 0, 'tcp_refused': 0, 'failed_batches': 0,
+                         'tcp_relayed': 0}
         self._lock = threading.Lock()                # one engine, two listener threads
         self.tcp = options.get('tcp', True)
         self._sock = None
@@ -172,6 +179,20 @@ class Server(object):
         deadline = None
         max_conns = self.options.get('max_tcp_conns', 1024)
         idle_s = self.options.get('tcp_idle_s', 30.0)
+        sink = wake_r = wake_w = None
+        if hasattr(self.recursion, 'submit') and hasattr(self.resolver, 'relay_batch'):
+            from .recursion import QueueSink
+            wake_r, wake_w = socket.socketpair()
+            wake_r.setblocking(False)
+            wake_w.setblocking(False)
+
+            def wake():
+                try:
+                    wake_w.send(b'\0')
+                except OSError:                      # full: a wake-up is pending anyway
+                    pass
+            sink = QueueSink(wake)
+            sel.register(wake_r, selectors.EVENT_READ)
 
         def close(s):
             c = conns.pop(s, None)
@@ -186,9 +207,13 @@ class Server(object):
             c = conns[s]
             ev = (0 if c.eof else selectors.EVENT_READ) | (selectors.EVENT_WRITE if c.outq else 0)
             if ev:
-                sel.modify(s, ev)
+                (sel.modify if c.reg else sel.register)(s, ev)
+                c.reg = True
             elif not c.waiting:                      # peer closed its side, nothing owed, nothing left to send
                 close(s)
+            elif c.reg:                              # half-closed and owed a relay: nothing to select on until it comes
+                sel.unregister(s)
+                c.reg = False
 
         last_sweep = time.perf_counter()
         while not self._stop.is_set():
@@ -200,6 +225,16 @@ class Server(object):
             now = time.perf_counter()
             for key, ev in events:
                 s = key.fileobj
+                if s is wake_r:
+                    try:
+                        while wake_r.recv(4096):
+                            pass
+                    except OSError:
+                        pass
+                    for item in sink.drain():
+                        for t in self._relay_tcp(item, conns):
+                            want(t)
+                    continue
                 if s is self._tsock:
                     try:
                         c, _ = self._tsock.accept()
@@ -247,7 +282,7 @@ class Server(object):
                 if s in conns:
                     want(s)
             if pending and (len(pending) >= self.max_batch or time.perf_counter() >= deadline):
-                self._resolve_and_send_tcp(pending, conns)
+                self._resolve_and_send_tcp(pending, conns, sink)
                 for s in set(ps for _, ps in pending):
                     if s in conns:
                         want(s)
@@ -259,8 +294,34 @@ class Server(object):
         for s in list(conns):
             close(s)
         sel.close()
+        if wake_r is not None:
+            wake_r.close()
+            wake_w.close()
 
-    def _resolve_and_send_tcp(self, pending, conns):
+    def _relay_tcp(self, item, conns):
+        """One window of relays drained from the TCP loop's sink: replies (tcp=True) appended to their connections, which
+        are owed one relay less each.  -> the connections still open"""
+        q_data, q_off, up, up_off, tags = item
+        with self._lock:
+            try:
+                res = self.resolver.relay_batch(q_data, q_off, up, up_off, tcp=True)
+            except Exception:                        # BinderError (capacity, CUDA): these misses get no replies
+                self.counters['failed_batches'] += 1
+                res = None
+        live = set()
+        for i, s in enumerate(tags):
+            c = conns.get(s)
+            if c is None:                            # closed meanwhile
+                continue
+            c.waiting -= 1
+            live.add(s)
+            if res is not None and res[3][i] == 0:
+                out, out_off, out_len, _ = res
+                c.outq += TcpFramer.frame(out[out_off[i]:out_off[i] + out_len[i]].tobytes())
+                self.counters['tcp_relayed'] += 1
+        return live
+
+    def _resolve_and_send_tcp(self, pending, conns, sink=None):
         pkts = [m for m, _ in pending]
         data, off = pack_packets(pkts)
         res = self._resolve(data, off, tcp=True)
@@ -282,8 +343,13 @@ class Server(object):
                 c['dropped'] += 1
         for i in miss:
             c['missed'] += 1
-            if self.recursion is not None:
-                self.recursion.resolve(pkts[int(i)], None, pending[int(i)][1])
+            s = pending[int(i)][1]
+            if sink is not None:
+                if s in conns:
+                    conns[s].waiting += 1
+                    self.recursion.submit(pkts[int(i)], sink, s)
+            elif self.recursion is not None:
+                self.recursion.resolve(pkts[int(i)], None, s)
 
     def _resolve_and_send(self, batch):
         pkts = [p for p, _ in batch if len(p) <= MAX_UDP]

@@ -441,6 +441,15 @@ int bb_shard_results(bb_shard* s, uint32_t src, const uint8_t** out, const uint3
  *                     a partial trailing frame is kept for the next call.  *out and the miss arrays point into the
  *                     session and stay valid until the next feed.  Handed-off misses (lib/server.js:110-113,222-225)
  *                     come back as packets + source addresses for the host's recursion.
+ *   bb_backend_relay  the session's replies to those misses, once the host's upstream exchange has an upstream response
+ *                     for each (q = the miss packets, up = upstream i, empty = the lookup failed): bb_relay_batch with
+ *                     flags 0 (the UDP path: 512-byte / EDNS limits) in batches of max_batch, then bb_frames_build: one
+ *                     OUTBOUND_UDP frame per answered relay, addressed to (dst_ip[i], dst_port[i]).  *out points into the
+ *                     session, valid until the next relay call; it does not invalidate bb_backend_feed's output.  Call
+ *                     it from the thread that feeds the session (they share its result buffers).  A failed batch
+ *                     (capacity, CUDA, an engine without `recursion`) loses its relays, counts them (stat 7) and the
+ *                     call goes on with the next batch; the return value is then the first batch's error.  BB_ERR_ARG
+ *                     for null arrays or decreasing offsets.
  */
 enum { BB_FRAME_CLIENT_HELLO = 1, BB_FRAME_INBOUND_UDP = 2, BB_FRAME_INBOUND_TCP = 3, BB_FRAME_CLIENT_HEARTBEAT = 4,
        BB_FRAME_SERVER_HELLO = 1001, BB_FRAME_OUTBOUND_UDP = 1002, BB_FRAME_INBOUND_TCP_OK = 1003, BB_FRAME_SERVER_HEARTBEAT = 1004 };
@@ -458,7 +467,12 @@ bb_backend* bb_backend_create(bb_engine* e, uint32_t max_batch, int* err);
 void        bb_backend_destroy(bb_backend* b);
 int         bb_backend_feed(bb_backend* b, const uint8_t* in, size_t in_len, uint64_t shuffle_seed,
                             const uint8_t** out, size_t* out_len, bb_backend_misses* misses);
-uint64_t    bb_backend_stat(const bb_backend* b, int what);   /* 0 udp frames 1 answered 2 missed 3 dropped 4 pending bytes 5 queries of failed batches */
+int         bb_backend_relay(bb_backend* b, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* up_pkts,
+                             const uint32_t* up_off, const uint32_t* dst_ip, const uint32_t* dst_port, uint32_t n,
+                             const uint8_t** out, size_t* out_len);
+/* 0 udp frames 1 answered 2 missed 3 dropped 4 pending bytes 5 queries of failed batches 6 replies relayed
+ * 7 queries of failed relay batches */
+uint64_t    bb_backend_stat(const bb_backend* b, int what);
 
 /* ---- mname-balancer TCP proxy sessions (deps/mname-balancer/backend.c:22-113, tcp_proxy.c:160-300) ----------------
  * The balancer hands every DNS-over-TCP client connection to a backend as its own AF_UNIX session.  The session opens
