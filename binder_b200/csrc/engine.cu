@@ -1023,6 +1023,14 @@ struct SlotCtx {
     PinnedCheck pinned;                          // of the caller's output sets
     uint8_t* out = nullptr; uint32_t out_cap = 0; uint32_t* miss_idx = nullptr; uint32_t* n_miss = nullptr;
 };
+// The device state of the calls on one stream (launches on different streams may overlap; on one stream they run in order):
+// the placement scratch, which every launch leaves zeroed, and the forward / match scratch (per-tile histograms, upstream
+// query lengths, the match's winner table), allocated on the first forward or match call.
+struct StreamCtx {
+    cudaStream_t stream = nullptr; unsigned long long* desc = nullptr;
+    unsigned long long* hist = nullptr; uint16_t* ulen = nullptr; uint32_t* win = nullptr;
+    void free_forward() { cudaFree(hist); cudaFree(ulen); cudaFree(win); }
+};
 }
 
 struct bb_engine {
@@ -1030,10 +1038,10 @@ struct bb_engine {
     bb::Slot* d_table = nullptr; uint8_t* d_arena = nullptr; uint32_t mask = 0; int ready = 0;
     int device = 0, ordered = 0; uint32_t max_batch = 0, max_bytes = 0, out_dev_cap = 0, max_tiles = 0;
     SlotCtx slots[NSLOTS];
-    // look-back / claim scratch of bb_resolve_batch_device, one per caller stream (launches on
-    // different streams may overlap)
+    // the device-form calls' contexts, one per caller stream; the synchronous calls' context borrows slot 0's stream and
+    // placement scratch
     static constexpr int MAX_DEV_STREAMS = 16;
-    void* dev_stream[MAX_DEV_STREAMS] = {}; unsigned long long* dev_desc[MAX_DEV_STREAMS] = {}; int n_dev_streams = 0;
+    StreamCtx dev[MAX_DEV_STREAMS], sync; int n_dev = 0;
     uint64_t launches = 0, epoch = 0;
     unsigned long long* stage_log = nullptr;
     // kernel variant per batch (bb_engine_set_kernel_profile): 0 = by the mean response size of the latest finished batch
@@ -1042,17 +1050,43 @@ struct bb_engine {
     uint32_t* h_fb = nullptr;
     // the zone this engine last synchronised with (incremental updates only continue from that state)
     const bb_zone* zone = nullptr; uint64_t zone_gen = 0; uint64_t arena_cap = 0;
-    // bb_relay_batch's device staging: allocated on first use, grown when a batch needs more (byte capacities)
-    struct RelayBuf { void* p = nullptr; size_t cap = 0; };
-    RelayBuf r_q, r_qoff, r_up, r_upoff, r_out, r_out_off, r_out_len, r_status, r_totals;
+    // the device staging of bb_relay_batch, bb_forward_batch and bb_match_upstreams (stage): one block for all three, as
+    // they run synchronously on slot 0's stream
+    uint8_t* staging = nullptr; size_t staging_cap = 0;
     PinnedCheck r_pinned;                        // of bb_relay_batch's output sets
-    // forward / match scratch (per-tile histograms, upstream query lengths, the match's winner table), one per stream
-    // like the look-back scratch: [MAX_DEV_STREAMS] = the synchronous calls' (slot 0's stream)
-    struct FwdScratch { unsigned long long* hist = nullptr; uint16_t* ulen = nullptr; uint32_t* win = nullptr; };
-    FwdScratch fwd[MAX_DEV_STREAMS + 1];
-    // bb_forward_batch / bb_match_upstreams device staging
-    RelayBuf f_pk, f_pkoff, f_uq, f_uqoff, f_order, f_goff, f_route, f_q, f_qoff, f_tot, f_resp, f_respoff, f_ip, f_port, f_up, f_upoff;
 };
+
+// A launch's placement scratch: desc[max_tiles] (each tile's published prefix), the arrival cursor in desc[max_tiles], the
+// claim counter in the word after it, and two spare words.
+static size_t place_scratch_bytes(const bb_engine* e) { return ((size_t)e->max_tiles + 4) * 8; }
+// The placement fields of a kernel's parameters (Params, RelayParams, FwdParams, MatchParams), with the launch's epoch.
+template <class P> static void place_params(bb_engine* e, unsigned long long* desc, P& p) {
+    p.desc = desc; p.counter = (uint32_t*)(desc + e->max_tiles + 1); p.ntiles_cap = e->max_tiles;
+    p.epoch = (uint32_t)(++e->epoch);
+}
+
+// One piece of the staging block: the device pointer it sets and the bytes it needs.
+struct Piece {
+    void** at; size_t bytes;
+    template <class T> Piece(T*& p, size_t n) : at((void**)&p), bytes(n) {}
+};
+// Cuts `pieces` out of the staging block in order, each 256-byte aligned as an allocation of its own would be; the block
+// grows (never shrinks) when they need more.  A kernel marks an overflow only by writing its epoch into totals[2], so every
+// call lists its totals first and a new block starts with them zeroed: that word never holds stale bytes of other pieces.
+static int stage(bb_engine* e, std::initializer_list<Piece> pieces) {
+    auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
+    size_t need = 0;
+    for (const Piece& p : pieces) need += up(p.bytes);
+    if (need > e->staging_cap) {
+        cudaFree(e->staging); e->staging = nullptr; e->staging_cap = 0;
+        CK(cudaMalloc(&e->staging, need));
+        CK(cudaMemsetAsync(e->staging, 0, 32, e->sync.stream));
+        e->staging_cap = need;
+    }
+    size_t at = 0;
+    for (const Piece& p : pieces) { *p.at = e->staging + at; at += up(p.bytes); }
+    return BB_OK;
+}
 
 // The zone and engine fields of the kernel parameters
 static void engine_params(const bb_engine* e, bbk::Params& P) {
@@ -1120,11 +1154,12 @@ static int engine_alloc(bb_engine* e) {
         CK(cudaMalloc(&s.d_out_len, (size_t)e->max_batch * 2 + 16));
         CK(cudaMalloc(&s.d_miss, (size_t)e->max_batch * 4 + 16));
         CK(cudaMalloc(&s.d_totals, 16));
-        CK(cudaMalloc(&s.d_desc, ((size_t)e->max_tiles + 4) * 8));
-        CK(cudaMemset(s.d_desc, 0, ((size_t)e->max_tiles + 4) * 8));
+        CK(cudaMalloc(&s.d_desc, place_scratch_bytes(e)));
+        CK(cudaMemset(s.d_desc, 0, place_scratch_bytes(e)));
         CK(cudaMemset(s.d_totals, 0, 16));
         CK(cudaMallocHost(&s.h_totals, 16));
     }
+    e->sync.stream = e->slots[0].stream; e->sync.desc = e->slots[0].d_desc;
     return BB_OK;
 }
 
@@ -1163,13 +1198,9 @@ void bb_engine_destroy(bb_engine* e) {
         cudaFree(s.d_miss); cudaFree(s.d_totals); cudaFree(s.d_desc); if (s.h_totals) cudaFreeHost(s.h_totals);
         if (s.ev) cudaEventDestroy(s.ev); if (s.stream) cudaStreamDestroy(s.stream);
     }
-    for (int i = 0; i < e->n_dev_streams; i++) cudaFree(e->dev_desc[i]);
-    for (auto* b : { &e->r_q, &e->r_qoff, &e->r_up, &e->r_upoff, &e->r_out, &e->r_out_off, &e->r_out_len, &e->r_status, &e->r_totals })
-        cudaFree(b->p);
-    for (auto* b : { &e->f_pk, &e->f_pkoff, &e->f_uq, &e->f_uqoff, &e->f_order, &e->f_goff, &e->f_route, &e->f_q, &e->f_qoff,
-                     &e->f_tot, &e->f_resp, &e->f_respoff, &e->f_ip, &e->f_port, &e->f_up, &e->f_upoff })
-        cudaFree(b->p);
-    for (auto& f : e->fwd) { cudaFree(f.hist); cudaFree(f.ulen); cudaFree(f.win); }
+    for (auto& c : e->dev) { cudaFree(c.desc); c.free_forward(); }
+    e->sync.free_forward();                      // its placement scratch is slot 0's
+    cudaFree(e->staging);
     cudaFree(e->d_const); cudaFree(e->d_table); cudaFree(e->d_arena);
     if (e->h_fb) cudaFreeHost(e->h_fb);
     delete e;
@@ -1276,8 +1307,7 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     P.out = d_out; P.out_cap = out_cap; P.out_off = d_out_off; P.out_len = d_out_len; P.status = d_status; P.miss_idx = d_miss; P.totals = d_totals;
     engine_params(e, P);
     P.ntiles = (n + bbk::T - 1) / bbk::T;
-    P.desc = desc; P.ntiles_cap = e->max_tiles; P.counter = (uint32_t*)(desc + e->max_tiles + 1);
-    P.epoch = (uint32_t)(++e->epoch);
+    place_params(e, desc, P);
     P.stage_log = e->stage_log;
     P.n_dev = nullptr; P.qidx_map = nullptr; P.route = 0; P.nranks = 1; P.rank = 0; P.regions = 0; P.bounce = bounce; P.qidx_out = nullptr; P.err_in = nullptr; P.tcp = (flags & BB_BATCH_TCP) ? 1u : 0u;
     // An empty batch still runs one block: its last-block path writes out_off[0] = 0 and totals {0, 0, -, epoch}, so a
@@ -1306,20 +1336,17 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     return BB_OK;
 }
 
-// The look-back / claim scratch of device-resident launches on `stream` (one per caller stream: launches on different
-// streams may overlap; launches on one stream run in order, and every launch leaves the scratch zeroed).
-static int stream_desc(bb_engine* e, void* stream, unsigned long long** desc) {
-    int si = -1;
-    for (int i = 0; i < e->n_dev_streams; i++) if (e->dev_stream[i] == stream) si = i;
-    if (si < 0) {
-        if (e->n_dev_streams == bb_engine::MAX_DEV_STREAMS) return BB_ERR_ARG;
-        CK(cudaSetDevice(e->device));
-        unsigned long long* dsc = nullptr;
-        CK(cudaMalloc(&dsc, ((size_t)e->max_tiles + 4) * 8));
-        CK(cudaMemset(dsc, 0, ((size_t)e->max_tiles + 4) * 8));
-        si = e->n_dev_streams++; e->dev_stream[si] = stream; e->dev_desc[si] = dsc;
-    }
-    *desc = e->dev_desc[si];
+// The context of the device-form calls on `stream` (all kinds share MAX_DEV_STREAMS), made on the stream's first call.
+static int stream_ctx(bb_engine* e, void* stream, StreamCtx** ctx) {
+    for (int i = 0; i < e->n_dev; i++)
+        if (e->dev[i].stream == (cudaStream_t)stream) { *ctx = &e->dev[i]; return BB_OK; }
+    if (e->n_dev == bb_engine::MAX_DEV_STREAMS) return BB_ERR_ARG;
+    StreamCtx& c = e->dev[e->n_dev];
+    CK(cudaSetDevice(e->device));
+    CK(cudaMalloc(&c.desc, place_scratch_bytes(e)));
+    CK(cudaMemset(c.desc, 0, place_scratch_bytes(e)));
+    c.stream = (cudaStream_t)stream; e->n_dev++;
+    *ctx = &c;
     return BB_OK;
 }
 
@@ -1328,11 +1355,11 @@ int bb_resolve_batch_device_ex(bb_engine* e, const uint8_t* d_pkts, const uint32
                                uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_miss_idx, uint32_t* d_totals, void* stream,
                                uint32_t flags) {
     if (!e || n > e->max_batch || ((uintptr_t)d_pkts & 15) || ((uintptr_t)d_out & 15)) return BB_ERR_ARG;
-    unsigned long long* desc = nullptr;
-    int rc = stream_desc(e, stream, &desc);
+    StreamCtx* c = nullptr;
+    int rc = stream_ctx(e, stream, &c);
     if (rc != BB_OK) return rc;
-    return launch(e, desc, d_pkts, d_pkt_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status, d_miss_idx,
-                  d_totals, (cudaStream_t)stream, nullptr, flags, true);
+    return launch(e, c->desc, d_pkts, d_pkt_off, n, seed, qidx_base, d_out, out_cap, d_out_off, d_out_len, d_status, d_miss_idx,
+                  d_totals, c->stream, nullptr, flags, true);
 }
 int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, uint32_t n,
                             uint64_t seed, uint32_t qidx_base, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
@@ -1342,74 +1369,67 @@ int bb_resolve_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t*
 }
 
 // ---- recursion relay (lib/recursion.js:287-327) -------------------------------------------------------------------
-static int relay_launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_q, const uint32_t* d_q_off, const uint8_t* d_up,
+static int relay_launch(bb_engine* e, const StreamCtx& c, const uint8_t* d_q, const uint32_t* d_q_off, const uint8_t* d_up,
                         const uint32_t* d_up_off, uint32_t n, uint32_t flags, uint8_t* out, uint32_t out_cap, uint32_t* out_off,
-                        uint16_t* out_len, uint8_t* status, uint32_t* totals, uint8_t* bounce, cudaStream_t st) {
+                        uint16_t* out_len, uint8_t* status, uint32_t* totals, uint8_t* bounce) {
     bbk::RelayParams P;
     P.q = d_q; P.q_off = d_q_off; P.up = d_up; P.up_off = d_up_off; P.n = n;
     P.out = out; P.out_cap = out_cap; P.out_off = out_off; P.out_len = out_len; P.status = status; P.totals = totals; P.bounce = bounce;
-    P.desc = desc; P.counter = (uint32_t*)(desc + e->max_tiles + 1); P.ntiles_cap = e->max_tiles;
-    P.epoch = (uint32_t)(++e->epoch); P.tcp = (flags & BB_BATCH_TCP) ? 1u : 0u;
+    place_params(e, c.desc, P); P.tcp = (flags & BB_BATCH_TCP) ? 1u : 0u;
     const uint32_t ntiles = (n + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;   // an empty batch still reports its totals
-    if (e->ordered) bbk::relay_kernel<true><<<grid, bbk::T, 0, st>>>(P);
-    else bbk::relay_kernel<false><<<grid, bbk::T, 0, st>>>(P);
+    if (e->ordered) bbk::relay_kernel<true><<<grid, bbk::T, 0, c.stream>>>(P);
+    else bbk::relay_kernel<false><<<grid, bbk::T, 0, c.stream>>>(P);
     CK(cudaGetLastError());
     e->launches++;
     return BB_OK;
 }
 
-static int relay_grow(bb_engine::RelayBuf& b, size_t need) {
-    if (need <= b.cap) return BB_OK;
-    cudaFree(b.p); b.p = nullptr; b.cap = 0;
-    CK(cudaMalloc(&b.p, need));
-    b.cap = need;
-    return BB_OK;
+// Whether off[0..n] never decreases.  No early exit, so that the compiler vectorises it: a batch has up to a million offsets.
+static bool offsets_ok(const uint32_t* off, uint32_t n) {
+    uint32_t bad = 0;
+    for (uint32_t i = 0; i < n; i++) bad |= off[i + 1] < off[i];
+    return !bad;
 }
 
 int bb_relay_batch(bb_engine* e, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* up_pkts, const uint32_t* up_off,
                    uint32_t n, uint32_t flags, uint8_t* out, uint32_t out_cap, uint32_t* out_off, uint16_t* out_len, uint8_t* status) {
     if (!e || !e->hconst.recursion || !q_off || !up_off || !out_off || n > e->max_batch) return BB_ERR_ARG;
-    if (n && (!status || !out_len || !out || (q_off[n] && !q_pkts) || (up_off[n] && !up_pkts))) return BB_ERR_ARG;
-    for (uint32_t i = 0; i < n; i++) if (q_off[i + 1] < q_off[i] || up_off[i + 1] < up_off[i]) return BB_ERR_ARG;
+    if (n && (!status || !out_len || !out || (q_off[n] && !q_pkts) || (up_off[n] && !up_pkts) || !offsets_ok(q_off, n) ||
+              !offsets_ok(up_off, n)))
+        return BB_ERR_ARG;
     const uint32_t qbytes = q_off[n], ubytes = up_off[n];
     const bool tcp = (flags & BB_BATCH_TCP) != 0;
     // a reply is at most 1,200 bytes over UDP and 65,535 over TCP: the device buffer never needs more than that per relay
     const uint64_t ocap = std::min<uint64_t>(out_cap, (uint64_t)n * (tcp ? 65535u : 1200u));
     CK(cudaSetDevice(e->device));
-    int rc;
-    if ((rc = relay_grow(e->r_q, (size_t)qbytes + 64)) || (rc = relay_grow(e->r_qoff, ((size_t)n + 1) * 4)) ||
-        (rc = relay_grow(e->r_up, (size_t)ubytes + 64)) || (rc = relay_grow(e->r_upoff, ((size_t)n + 1) * 4)) ||
-        (rc = relay_grow(e->r_out, (size_t)ocap + 64)) || (rc = relay_grow(e->r_totals, 16)))
-        return rc;
-    // zero-copy results when every output buffer is pinned host memory (bb_host_alloc), as bb_resolve_submit_ex does
+    // zero-copy results when every output buffer is pinned host memory (bb_host_alloc), as bb_resolve_submit_ex does: the
+    // device output is then the kernel's bounce buffer, and the offsets, lengths and statuses need no device copy
     const void* outs[4] = { out, out_off, out_len, status };
     const bool zc = e->r_pinned.check(outs, 4) && n != 0;
-    if (!zc && ((rc = relay_grow(e->r_out_off, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->r_out_len, (size_t)n * 2 + 16)) ||
-                (rc = relay_grow(e->r_status, (size_t)n + 16))))
-        return rc;
-    SlotCtx& s = e->slots[0];                    // the stream (and look-back state) of the synchronous resolve calls
-    if (qbytes) CK(cudaMemcpyAsync(e->r_q.p, q_pkts, qbytes, cudaMemcpyHostToDevice, s.stream));
-    if (ubytes) CK(cudaMemcpyAsync(e->r_up.p, up_pkts, ubytes, cudaMemcpyHostToDevice, s.stream));
-    CK(cudaMemcpyAsync(e->r_qoff.p, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, s.stream));
-    CK(cudaMemcpyAsync(e->r_upoff.p, up_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, s.stream));
-    uint8_t* d_out = (uint8_t*)e->r_out.p;
-    rc = zc ? relay_launch(e, s.d_desc, (uint8_t*)e->r_q.p, (uint32_t*)e->r_qoff.p, (uint8_t*)e->r_up.p, (uint32_t*)e->r_upoff.p, n, flags,
-                           out, (uint32_t)ocap, out_off, out_len, status, (uint32_t*)e->r_totals.p, d_out, s.stream)
-            : relay_launch(e, s.d_desc, (uint8_t*)e->r_q.p, (uint32_t*)e->r_qoff.p, (uint8_t*)e->r_up.p, (uint32_t*)e->r_upoff.p, n, flags,
-                           d_out, (uint32_t)ocap, (uint32_t*)e->r_out_off.p, (uint16_t*)e->r_out_len.p, (uint8_t*)e->r_status.p,
-                           (uint32_t*)e->r_totals.p, nullptr, s.stream);
+    uint8_t *d_q, *d_up, *d_out, *d_status; uint32_t *d_totals, *d_qoff, *d_upoff, *d_out_off; uint16_t* d_out_len;
+    int rc = stage(e, { { d_totals, 16 }, { d_q, (size_t)qbytes + 64 }, { d_qoff, ((size_t)n + 1) * 4 }, { d_up, (size_t)ubytes + 64 },
+                        { d_upoff, ((size_t)n + 1) * 4 }, { d_out, (size_t)ocap + 64 }, { d_out_off, zc ? 0 : ((size_t)n + 1) * 4 },
+                        { d_out_len, zc ? 0 : (size_t)n * 2 + 16 }, { d_status, zc ? 0 : (size_t)n + 16 } });
+    if (rc != BB_OK) return rc;
+    const StreamCtx& c = e->sync;
+    if (qbytes) CK(cudaMemcpyAsync(d_q, q_pkts, qbytes, cudaMemcpyHostToDevice, c.stream));
+    if (ubytes) CK(cudaMemcpyAsync(d_up, up_pkts, ubytes, cudaMemcpyHostToDevice, c.stream));
+    CK(cudaMemcpyAsync(d_qoff, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
+    CK(cudaMemcpyAsync(d_upoff, up_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
+    rc = relay_launch(e, c, d_q, d_qoff, d_up, d_upoff, n, flags, zc ? out : d_out, (uint32_t)ocap, zc ? out_off : d_out_off,
+                      zc ? out_len : d_out_len, zc ? status : d_status, d_totals, zc ? d_out : nullptr);
     if (rc != BB_OK) return rc;
     const uint32_t epoch = (uint32_t)e->epoch;
     uint32_t tot[4];
-    CK(cudaMemcpyAsync(tot, e->r_totals.p, 16, cudaMemcpyDeviceToHost, s.stream));
-    CK(cudaStreamSynchronize(s.stream));
+    CK(cudaMemcpyAsync(tot, d_totals, 16, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
     if (tot[2] == epoch || tot[0] > out_cap) return BB_ERR_CAPACITY;
     if (zc) return BB_OK;                        // everything is already in the caller's buffers
-    if (tot[0]) CK(cudaMemcpyAsync(out, d_out, tot[0], cudaMemcpyDeviceToHost, s.stream));
-    CK(cudaMemcpyAsync(out_off, e->r_out_off.p, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, s.stream));
-    if (n) CK(cudaMemcpyAsync(out_len, e->r_out_len.p, (size_t)n * 2, cudaMemcpyDeviceToHost, s.stream));
-    if (n) CK(cudaMemcpyAsync(status, e->r_status.p, n, cudaMemcpyDeviceToHost, s.stream));
-    CK(cudaStreamSynchronize(s.stream));
+    if (tot[0]) CK(cudaMemcpyAsync(out, d_out, tot[0], cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaMemcpyAsync(out_off, d_out_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
+    if (n) CK(cudaMemcpyAsync(out_len, d_out_len, (size_t)n * 2, cudaMemcpyDeviceToHost, c.stream));
+    if (n) CK(cudaMemcpyAsync(status, d_status, n, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
     return BB_OK;
 }
 
@@ -1418,33 +1438,23 @@ int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t*
                           uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_totals, void* stream) {
     if (!e || !e->hconst.recursion || n > e->max_batch || ((uintptr_t)d_q_pkts & 15) || ((uintptr_t)d_up_pkts & 15) || ((uintptr_t)d_out & 15))
         return BB_ERR_ARG;
-    unsigned long long* desc = nullptr;
-    int rc = stream_desc(e, stream, &desc);
+    StreamCtx* c = nullptr;
+    int rc = stream_ctx(e, stream, &c);
     if (rc != BB_OK) return rc;
-    return relay_launch(e, desc, d_q_pkts, d_q_off, d_up_pkts, d_up_off, n, flags, d_out, out_cap, d_out_off, d_out_len, d_status,
-                        d_totals, nullptr, (cudaStream_t)stream);
+    return relay_launch(e, *c, d_q_pkts, d_q_off, d_up_pkts, d_up_off, n, flags, d_out, out_cap, d_out_off, d_out_len, d_status,
+                        d_totals, nullptr);
 }
 
 // ---- recursion forward and match (lib/recursion.js:253-280,335-354,382-387) --------------------------------------------
 static bool forward_ready(const bb_engine* e) { return e && e->hconst.recursion == 2 && e->hconst.fu_n; }
-// Look-back and forward scratch of `stream` (NULL `stream` with `sync`: the synchronous calls' own, on slot 0's stream).
-static int fwd_scratch(bb_engine* e, void* stream, bool sync, unsigned long long** desc, bb_engine::FwdScratch** fs) {
-    int si = bb_engine::MAX_DEV_STREAMS;
-    if (sync) *desc = e->slots[0].d_desc;
-    else {
-        int rc = stream_desc(e, stream, desc);
-        if (rc != BB_OK) return rc;
-        for (int i = 0; i < e->n_dev_streams; i++) if (e->dev_stream[i] == stream) si = i;
-    }
-    bb_engine::FwdScratch& f = e->fwd[si];
-    if (!f.hist) {
-        CK(cudaSetDevice(e->device));
-        CK(cudaMalloc(&f.hist, (size_t)(bbk::FWD_MAX / bbk::T) * bbk::NROUTE * 8));
-        CK(cudaMalloc(&f.ulen, (size_t)bbk::FWD_MAX * 2));
-        CK(cudaMalloc(&f.win, (size_t)bbk::FWD_MAX * 4));
-        CK(cudaMemset(f.win, 0xFF, (size_t)bbk::FWD_MAX * 4));       // NO_MATCH; match_gather_kernel leaves it so
-    }
-    *fs = &f;
+// The forward / match scratch of context `c`, allocated on its first forward or match call.
+static int forward_scratch(bb_engine* e, StreamCtx& c) {
+    if (c.hist) return BB_OK;
+    CK(cudaSetDevice(e->device));
+    CK(cudaMalloc(&c.hist, (size_t)(bbk::FWD_MAX / bbk::T) * bbk::NROUTE * 8));
+    CK(cudaMalloc(&c.ulen, (size_t)bbk::FWD_MAX * 2));
+    CK(cudaMalloc(&c.win, (size_t)bbk::FWD_MAX * 4));
+    CK(cudaMemset(c.win, 0xFF, (size_t)bbk::FWD_MAX * 4));           // NO_MATCH; match_gather_kernel leaves it so
     return BB_OK;
 }
 // the misses one forward / match launch covers: the engine's look-back scratch holds max_tiles tiles
@@ -1452,48 +1462,45 @@ static uint32_t fwd_cap(const bb_engine* e, uint32_t n_cap) {
     return std::min(std::min(n_cap, bbk::FWD_MAX), e->max_tiles * (uint32_t)bbk::T);
 }
 
-static int forward_launch(bb_engine* e, unsigned long long* desc, bb_engine::FwdScratch* fs, const uint8_t* pkts, const uint32_t* pkt_off,
+static int forward_launch(bb_engine* e, StreamCtx& c, const uint8_t* pkts, const uint32_t* pkt_off,
                           const uint32_t* miss_idx, const uint32_t* n_dev, uint32_t n, uint32_t n_cap, uint64_t id_key,
                           uint8_t* uq, uint32_t uq_cap, uint32_t* uq_off, uint32_t* order, uint32_t* group_off, uint8_t* route,
-                          uint8_t* q, uint32_t q_cap, uint32_t* q_off, uint32_t* totals, cudaStream_t st) {
+                          uint8_t* q, uint32_t q_cap, uint32_t* q_off, uint32_t* totals) {
+    int rc = forward_scratch(e, c);
+    if (rc != BB_OK) return rc;
     bbk::FwdParams P;
     P.pkts = pkts; P.pkt_off = pkt_off; P.miss_idx = miss_idx; P.n_dev = n_dev; P.n = n; P.n_cap = n_cap;
     P.eng = e->d_const; P.key = bbk::id_key_rounds(id_key);
     P.uq = uq; P.uq_cap = uq_cap; P.uq_off = uq_off; P.order = order; P.group_off = group_off; P.route = route;
-    P.q = q; P.q_cap = q_cap; P.q_off = q_off; P.totals = totals; P.hist = fs->hist; P.ulen = fs->ulen;
-    P.desc = desc; P.counter = (uint32_t*)(desc + e->max_tiles + 1); P.ntiles_cap = e->max_tiles;
-    P.epoch = (uint32_t)(++e->epoch);
+    P.q = q; P.q_cap = q_cap; P.q_off = q_off; P.totals = totals; P.hist = c.hist; P.ulen = c.ulen;
+    place_params(e, c.desc, P);
     const uint32_t ntiles = (n_cap + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;     // an empty call still reports its totals
-    bbk::forward_kernel<<<grid, bbk::T, 0, st>>>(P);
-    bbk::forward_group_kernel<<<1, bbk::FG_T, 0, st>>>(P);
-    bbk::forward_scatter_kernel<<<grid, bbk::T, 0, st>>>(P);
+    bbk::forward_kernel<<<grid, bbk::T, 0, c.stream>>>(P);
+    bbk::forward_group_kernel<<<1, bbk::FG_T, 0, c.stream>>>(P);
+    bbk::forward_scatter_kernel<<<grid, bbk::T, 0, c.stream>>>(P);
     CK(cudaGetLastError());
     e->launches += 3;
     return BB_OK;
 }
 
-static int match_launch(bb_engine* e, unsigned long long* desc, bb_engine::FwdScratch* fs, const uint8_t* resp, const uint32_t* resp_off,
+static int match_launch(bb_engine* e, StreamCtx& c, const uint8_t* resp, const uint32_t* resp_off,
                         const uint32_t* src_ip, const uint16_t* src_port, uint32_t n_resp, const uint8_t* q, const uint32_t* q_off,
                         const uint8_t* route, const uint32_t* n_dev, uint32_t n, uint32_t n_cap, uint64_t id_key, uint8_t* up,
-                        uint32_t up_cap, uint32_t* up_off, uint32_t* totals, cudaStream_t st) {
+                        uint32_t up_cap, uint32_t* up_off, uint32_t* totals) {
+    int rc = forward_scratch(e, c);
+    if (rc != BB_OK) return rc;
     bbk::MatchParams P;
     P.resp = resp; P.resp_off = resp_off; P.src_ip = src_ip; P.src_port = src_port; P.n_resp = n_resp;
     P.c = q; P.c_off = q_off; P.route = route; P.n_dev = n_dev; P.n = n; P.n_cap = n_cap;
-    P.eng = e->d_const; P.key = bbk::id_key_rounds(id_key); P.win = fs->win;
+    P.eng = e->d_const; P.key = bbk::id_key_rounds(id_key); P.win = c.win;
     P.up = up; P.up_cap = up_cap; P.up_off = up_off; P.totals = totals;
-    P.desc = desc; P.counter = (uint32_t*)(desc + e->max_tiles + 1); P.ntiles_cap = e->max_tiles;
-    P.epoch = (uint32_t)(++e->epoch);
-    if (n_resp) bbk::match_kernel<<<(n_resp + 255) / 256, 256, 0, st>>>(P);
+    place_params(e, c.desc, P);
+    if (n_resp) bbk::match_kernel<<<(n_resp + 255) / 256, 256, 0, c.stream>>>(P);
     const uint32_t ntiles = (n_cap + bbk::T - 1) / bbk::T;
-    bbk::match_gather_kernel<<<ntiles ? ntiles : 1u, bbk::T, 0, st>>>(P);
+    bbk::match_gather_kernel<<<ntiles ? ntiles : 1u, bbk::T, 0, c.stream>>>(P);
     CK(cudaGetLastError());
     e->launches += n_resp ? 2 : 1;
     return BB_OK;
-}
-
-static bool offsets_ok(const uint32_t* off, uint32_t n) {
-    for (uint32_t i = 0; i < n; i++) if (off[i + 1] < off[i]) return false;
-    return true;
 }
 
 int bb_forward_batch(bb_engine* e, const uint8_t* pkts, const uint32_t* pkt_off, uint32_t n, uint64_t id_key, uint8_t* uq,
@@ -1502,35 +1509,30 @@ int bb_forward_batch(bb_engine* e, const uint8_t* pkts, const uint32_t* pkt_off,
     if (n && (!order || !route || !uq || (pkt_off[n] && !pkts) || !offsets_ok(pkt_off, n))) return BB_ERR_ARG;
     const uint32_t bytes = pkt_off[n];
     CK(cudaSetDevice(e->device));
-    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
-    int rc;
-    if ((rc = fwd_scratch(e, nullptr, true, &desc, &fs)) || (rc = relay_grow(e->f_pk, (size_t)bytes + 64)) ||
-        (rc = relay_grow(e->f_pkoff, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->f_uq, (size_t)bytes + 64)) ||
-        (rc = relay_grow(e->f_uqoff, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->f_order, (size_t)n * 4 + 16)) ||
-        (rc = relay_grow(e->f_goff, (bbk::NROUTE + 1) * 4)) || (rc = relay_grow(e->f_route, (size_t)n + 16)) ||
-        (rc = relay_grow(e->f_q, (size_t)bytes + 64)) || (rc = relay_grow(e->f_qoff, ((size_t)n + 1) * 4)) ||
-        (rc = relay_grow(e->f_tot, 32)))
-        return rc;
-    cudaStream_t st = e->slots[0].stream;
-    if (bytes) CK(cudaMemcpyAsync(e->f_pk.p, pkts, bytes, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->f_pkoff.p, pkt_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
+    uint8_t *d_pk, *d_uq, *d_route, *d_q; uint32_t *d_tot, *d_pkoff, *d_uqoff, *d_order, *d_goff, *d_qoff;
+    int rc = stage(e, { { d_tot, 32 }, { d_pk, (size_t)bytes + 64 }, { d_pkoff, ((size_t)n + 1) * 4 }, { d_uq, (size_t)bytes + 64 },
+                        { d_uqoff, ((size_t)n + 1) * 4 }, { d_order, (size_t)n * 4 + 16 }, { d_goff, (bbk::NROUTE + 1) * 4 },
+                        { d_route, (size_t)n + 16 }, { d_q, (size_t)bytes + 64 }, { d_qoff, ((size_t)n + 1) * 4 } });
+    if (rc != BB_OK) return rc;
+    StreamCtx& c = e->sync;
+    if (bytes) CK(cudaMemcpyAsync(d_pk, pkts, bytes, cudaMemcpyHostToDevice, c.stream));
+    CK(cudaMemcpyAsync(d_pkoff, pkt_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
     // an upstream query is never longer than its client query: the device buffers hold the whole batch
-    rc = forward_launch(e, desc, fs, (uint8_t*)e->f_pk.p, (uint32_t*)e->f_pkoff.p, nullptr, nullptr, n, n, id_key, (uint8_t*)e->f_uq.p,
-                        bytes, (uint32_t*)e->f_uqoff.p, (uint32_t*)e->f_order.p, (uint32_t*)e->f_goff.p, (uint8_t*)e->f_route.p,
-                        (uint8_t*)e->f_q.p, bytes, (uint32_t*)e->f_qoff.p, (uint32_t*)e->f_tot.p, st);
+    rc = forward_launch(e, c, d_pk, d_pkoff, nullptr, nullptr, n, n, id_key, d_uq, bytes, d_uqoff, d_order, d_goff, d_route, d_q, bytes,
+                        d_qoff, d_tot);
     if (rc != BB_OK) return rc;
     const uint32_t epoch = (uint32_t)e->epoch;
     uint32_t tot[5];
-    CK(cudaMemcpyAsync(tot, e->f_tot.p, 20, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(tot, d_tot, 20, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
     if (tot[2] == epoch) { g_cuda_err = "forward: device buffers overflowed"; return BB_ERR_CUDA; }
     if (tot[0] > uq_cap) return BB_ERR_CAPACITY;
-    if (tot[0]) CK(cudaMemcpyAsync(uq, e->f_uq.p, tot[0], cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(uq_off, e->f_uqoff.p, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(group_off, e->f_goff.p, (bbk::NROUTE + 1) * 4, cudaMemcpyDeviceToHost, st));
-    if (n) CK(cudaMemcpyAsync(order, e->f_order.p, (size_t)n * 4, cudaMemcpyDeviceToHost, st));
-    if (n) CK(cudaMemcpyAsync(route, e->f_route.p, n, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    if (tot[0]) CK(cudaMemcpyAsync(uq, d_uq, tot[0], cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaMemcpyAsync(uq_off, d_uqoff, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaMemcpyAsync(group_off, d_goff, (bbk::NROUTE + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
+    if (n) CK(cudaMemcpyAsync(order, d_order, (size_t)n * 4, cudaMemcpyDeviceToHost, c.stream));
+    if (n) CK(cudaMemcpyAsync(route, d_route, n, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
     return BB_OK;
 }
 
@@ -1541,11 +1543,11 @@ int bb_forward_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t*
     if (!forward_ready(e) || !d_pkts || !d_pkt_off || !d_miss_idx || !d_resolve_totals || !d_uq || !d_uq_off || !d_order ||
         !d_group_off || !d_route || !d_q || !d_q_off || !d_totals)
         return BB_ERR_ARG;
-    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
-    int rc = fwd_scratch(e, stream, false, &desc, &fs);
+    StreamCtx* c = nullptr;
+    int rc = stream_ctx(e, stream, &c);
     if (rc != BB_OK) return rc;
-    return forward_launch(e, desc, fs, d_pkts, d_pkt_off, d_miss_idx, d_resolve_totals, 0, fwd_cap(e, n_cap), id_key, d_uq, uq_cap,
-                          d_uq_off, d_order, d_group_off, d_route, d_q, q_cap, d_q_off, d_totals, (cudaStream_t)stream);
+    return forward_launch(e, *c, d_pkts, d_pkt_off, d_miss_idx, d_resolve_totals, 0, fwd_cap(e, n_cap), id_key, d_uq, uq_cap,
+                          d_uq_off, d_order, d_group_off, d_route, d_q, q_cap, d_q_off, d_totals);
 }
 
 int bb_match_upstreams(bb_engine* e, const uint8_t* resp, const uint32_t* resp_off, const uint32_t* src_ip, const uint16_t* src_port,
@@ -1557,35 +1559,31 @@ int bb_match_upstreams(bb_engine* e, const uint8_t* resp, const uint32_t* resp_o
     if (n && (!route || (q_off[n] && !q_pkts) || !offsets_ok(q_off, n))) return BB_ERR_ARG;
     const uint32_t rbytes = resp_off[n_resp], qbytes = q_off[n];
     CK(cudaSetDevice(e->device));
-    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
-    int rc;
-    if ((rc = fwd_scratch(e, nullptr, true, &desc, &fs)) || (rc = relay_grow(e->f_resp, (size_t)rbytes + 64)) ||
-        (rc = relay_grow(e->f_respoff, ((size_t)n_resp + 1) * 4)) || (rc = relay_grow(e->f_ip, (size_t)n_resp * 4 + 16)) ||
-        (rc = relay_grow(e->f_port, (size_t)n_resp * 2 + 16)) || (rc = relay_grow(e->f_q, (size_t)qbytes + 64)) ||
-        (rc = relay_grow(e->f_qoff, ((size_t)n + 1) * 4)) || (rc = relay_grow(e->f_route, (size_t)n + 16)) ||
-        (rc = relay_grow(e->f_up, (size_t)rbytes + 64)) || (rc = relay_grow(e->f_upoff, ((size_t)n + 1) * 4)) ||
-        (rc = relay_grow(e->f_tot, 32)))
-        return rc;
-    cudaStream_t st = e->slots[0].stream;
-    if (rbytes) CK(cudaMemcpyAsync(e->f_resp.p, resp, rbytes, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->f_respoff.p, resp_off, ((size_t)n_resp + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (n_resp) CK(cudaMemcpyAsync(e->f_ip.p, src_ip, (size_t)n_resp * 4, cudaMemcpyHostToDevice, st));
-    if (n_resp) CK(cudaMemcpyAsync(e->f_port.p, src_port, (size_t)n_resp * 2, cudaMemcpyHostToDevice, st));
-    if (qbytes) CK(cudaMemcpyAsync(e->f_q.p, q_pkts, qbytes, cudaMemcpyHostToDevice, st));
-    CK(cudaMemcpyAsync(e->f_qoff.p, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, st));
-    if (n) CK(cudaMemcpyAsync(e->f_route.p, route, n, cudaMemcpyHostToDevice, st));
+    uint8_t *d_resp, *d_q, *d_route, *d_up; uint32_t *d_tot, *d_respoff, *d_ip, *d_qoff, *d_upoff; uint16_t* d_port;
+    int rc = stage(e, { { d_tot, 32 }, { d_resp, (size_t)rbytes + 64 }, { d_respoff, ((size_t)n_resp + 1) * 4 },
+                        { d_ip, (size_t)n_resp * 4 + 16 }, { d_port, (size_t)n_resp * 2 + 16 }, { d_q, (size_t)qbytes + 64 },
+                        { d_qoff, ((size_t)n + 1) * 4 }, { d_route, (size_t)n + 16 }, { d_up, (size_t)rbytes + 64 },
+                        { d_upoff, ((size_t)n + 1) * 4 } });
+    if (rc != BB_OK) return rc;
+    StreamCtx& c = e->sync;
+    if (rbytes) CK(cudaMemcpyAsync(d_resp, resp, rbytes, cudaMemcpyHostToDevice, c.stream));
+    CK(cudaMemcpyAsync(d_respoff, resp_off, ((size_t)n_resp + 1) * 4, cudaMemcpyHostToDevice, c.stream));
+    if (n_resp) CK(cudaMemcpyAsync(d_ip, src_ip, (size_t)n_resp * 4, cudaMemcpyHostToDevice, c.stream));
+    if (n_resp) CK(cudaMemcpyAsync(d_port, src_port, (size_t)n_resp * 2, cudaMemcpyHostToDevice, c.stream));
+    if (qbytes) CK(cudaMemcpyAsync(d_q, q_pkts, qbytes, cudaMemcpyHostToDevice, c.stream));
+    CK(cudaMemcpyAsync(d_qoff, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
+    if (n) CK(cudaMemcpyAsync(d_route, route, n, cudaMemcpyHostToDevice, c.stream));
     // the winners are distinct responses: their bytes fit a buffer of all the responses
-    rc = match_launch(e, desc, fs, (uint8_t*)e->f_resp.p, (uint32_t*)e->f_respoff.p, (uint32_t*)e->f_ip.p, (uint16_t*)e->f_port.p, n_resp,
-                      (uint8_t*)e->f_q.p, (uint32_t*)e->f_qoff.p, (uint8_t*)e->f_route.p, nullptr, n, n, id_key, (uint8_t*)e->f_up.p,
-                      rbytes, (uint32_t*)e->f_upoff.p, (uint32_t*)e->f_tot.p, st);
+    rc = match_launch(e, c, d_resp, d_respoff, d_ip, d_port, n_resp, d_q, d_qoff, d_route, nullptr, n, n, id_key, d_up, rbytes, d_upoff,
+                      d_tot);
     if (rc != BB_OK) return rc;
     uint32_t tot[4];
-    CK(cudaMemcpyAsync(tot, e->f_tot.p, 16, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    CK(cudaMemcpyAsync(tot, d_tot, 16, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
     if (tot[0] > up_cap) return BB_ERR_CAPACITY;
-    if (tot[0]) CK(cudaMemcpyAsync(up, e->f_up.p, tot[0], cudaMemcpyDeviceToHost, st));
-    CK(cudaMemcpyAsync(up_off, e->f_upoff.p, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    if (tot[0]) CK(cudaMemcpyAsync(up, d_up, tot[0], cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaMemcpyAsync(up_off, d_upoff, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
     return BB_OK;
 }
 
@@ -1596,11 +1594,11 @@ int bb_match_upstreams_device(bb_engine* e, const uint8_t* d_resp, const uint32_
     if (!forward_ready(e) || n_resp > BB_MATCH_MAX_RESPONSES || !d_resp_off || (n_resp && (!d_resp || !d_src_ip || !d_src_port)) ||
         !d_q || !d_q_off || !d_route || !d_forward_totals || !d_up || !d_up_off || !d_totals)
         return BB_ERR_ARG;
-    unsigned long long* desc = nullptr; bb_engine::FwdScratch* fs = nullptr;
-    int rc = fwd_scratch(e, stream, false, &desc, &fs);
+    StreamCtx* c = nullptr;
+    int rc = stream_ctx(e, stream, &c);
     if (rc != BB_OK) return rc;
-    return match_launch(e, desc, fs, d_resp, d_resp_off, d_src_ip, d_src_port, n_resp, d_q, d_q_off, d_route, d_forward_totals, 0,
-                        fwd_cap(e, n_cap), id_key, d_up, up_cap, d_up_off, d_totals, (cudaStream_t)stream);
+    return match_launch(e, *c, d_resp, d_resp_off, d_src_ip, d_src_port, n_resp, d_q, d_q_off, d_route, d_forward_totals, 0,
+                        fwd_cap(e, n_cap), id_key, d_up, up_cap, d_up_off, d_totals);
 }
 
 int bb_resolve_submit_ex(bb_engine* e, int slot, const uint8_t* pkts, const uint32_t* pkt_off, uint32_t n, uint64_t seed,
@@ -1731,7 +1729,7 @@ bb_shard* bb_shard_create(bb_engine* e, uint32_t nranks, uint32_t rank, uint32_t
     auto ck = [&](cudaError_t c) { if (c != cudaSuccess) { g_cuda_err = cudaGetErrorString(c); return false; } return true; };
     auto up = [](size_t v) { return (v + 255) & ~(size_t)255; };
     s->out_stride = up((size_t)s->out_cap + 64); s->off_stride = up(((size_t)s->cap_q + 1) * 4); s->len_stride = up((size_t)s->cap_q * 2 + 16);
-    s->status_stride = up((size_t)s->cap_q + 16); s->miss_stride = up((size_t)s->cap_q * 4 + 16); s->desc_stride = up(((size_t)e->max_tiles + 4) * 8);
+    s->status_stride = up((size_t)s->cap_q + 16); s->miss_stride = up((size_t)s->cap_q * 4 + 16); s->desc_stride = up(place_scratch_bytes(e));
     bool ok = ck(cudaSetDevice(e->device)) && ck(cudaMalloc(&s->recv, s->reg_size * nranks * 2)) && ck(cudaMemset(s->recv, 0, s->reg_size * nranks * 2)) &&
               ck(cudaMalloc(&s->cursor, 8 * bbk::MAX_RANKS)) && ck(cudaMemset(s->cursor, 0, 8 * bbk::MAX_RANKS)) &&
               ck(cudaMalloc(&s->done, 16)) && ck(cudaMemset(s->done, 0, 16)) &&
@@ -1866,9 +1864,9 @@ int bb_shard_resolve(bb_shard* s, uint64_t seed, int wait_for_peers, void* strea
         P.bounce = s->d_out;                         // tiles too large to stage assemble on the device first
     }
     engine_params(e, P);
-    P.ntiles = (s->cap_q + bbk::T - 1) / bbk::T; P.ntiles_cap = e->max_tiles;
-    P.desc = (unsigned long long*)s->d_desc; P.counter = (uint32_t*)((unsigned long long*)s->d_desc + e->max_tiles + 1);
-    P.epoch = (uint32_t)(++e->epoch); P.stage_log = nullptr; P.route = 0; P.nranks = s->nranks; P.rank = s->rank;
+    P.ntiles = (s->cap_q + bbk::T - 1) / bbk::T;
+    place_params(e, (unsigned long long*)s->d_desc, P);
+    P.stage_log = nullptr; P.route = 0; P.nranks = s->nranks; P.rank = s->rank;
     P.regions = 1; P.in_stride = s->reg_size; P.out_stride = s->out_stride; P.off_stride = s->off_stride; P.len_stride = s->len_stride;
     P.status_stride = s->status_stride; P.miss_stride = s->miss_stride; P.totals_stride = s->totals_stride; P.desc_stride = s->desc_stride;
     resolve_launch(P, dim3(P.ntiles, s->nranks), main, e->ordered, false);
