@@ -403,8 +403,10 @@ __device__ __forceinline__ void size_single(Res& r, uint32_t fixed, uint32_t rr)
 
 // Recursion.resolve()'s quick rejects (lib/recursion.js:329-344), for a miss that would otherwise be handed
 // to the host: would it be forwarded anywhere?  nm = QNAME wire bytes — query.name() in its original case,
-// SRV prefix included — W = its length without the terminator.  In the dotted string every label boundary
-// is a '.', so the string operations map one to one onto wire positions:
+// SRV prefix included — W = its length without the terminator.  The dotted string is the wire bytes with each
+// label boundary written as a '.', so the string operations map one to one onto wire positions; a '.' inside a
+// label is a '.' of that string like any other (query.name() does not escape it), both in the suffix compare and
+// as the start of dc:
 //   domain.indexOf(dnsDomain, domain.length - dnsDomain.length) === -1            -> not ours   (:330-333)
 //   p = domain minus the suffix and the one character before it; dc = p after its last '.';
 //   self.dcs[dc] === undefined (or every upstream of dc is this host)              -> nowhere to ask (:338-343,377-379)
@@ -419,15 +421,13 @@ __device__ __forceinline__ int rf_scan(const EngineConst* E, const uint8_t* nm, 
     const uint32_t s0 = W - L;                         // wire index where the suffix must start
     if (s0 < 2) return NO;                             // nothing before it: dc = ''
     const uint32_t cw = s0 - 1;                        // the character substring() drops (normally the '.')
-    uint32_t nlp = 1u + nm[0], last_b = 0;             // next length byte; last boundary before cw
+    uint32_t nlp = 1u + nm[0], last_b = 0;             // next length byte; last '.' of the dotted string before cw
     bool ok = true;
     for (uint32_t w = 1; w < W; w++) {
         const bool boundary = w == nlp;
-        if (boundary) { nlp = w + 1u + nm[w]; if (w < cw) last_b = w; }
-        if (w >= s0) {
-            const uint32_t e = E->rf_dom[w - s0];
-            ok &= boundary ? e == '.' : (e != '.' && e == nm[w]);
-        }
+        if (boundary) nlp = w + 1u + nm[w];
+        if ((boundary || nm[w] == '.') && w < cw) last_b = w;
+        if (w >= s0) ok &= E->rf_dom[w - s0] == (boundary ? (uint8_t)'.' : nm[w]);
     }
     if (!ok) return NO;
     const uint32_t d0 = last_b + 1, dl = cw - d0;      // dc = dotted[d0 .. cw)

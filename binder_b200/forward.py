@@ -50,6 +50,8 @@ class GpuRecursion(object):
         resolver.set_recursion_upstreams(table)
         self.timeout = timeout
         self.window_s = window_s
+        # misses per window: the 16-bit ID space, and no more than one forward / match / relay call of the resolver takes
+        self.window_max = min(FORWARD_MAX, getattr(resolver, 'max_batch', FORWARD_MAX))
         self.counters = {'relayed': 0, 'forwarded': 0, 'upstream_answers': 0, 'tcp_skipped': 0, 'failed_batches': 0,
                          'delivered': 0}
         self._udp = UdpSink(resolver, self.counters)
@@ -80,7 +82,7 @@ class GpuRecursion(object):
             except queue.Empty:
                 continue
             deadline = time.perf_counter() + self.window_s
-            while time.perf_counter() < deadline and len(batch) < FORWARD_MAX:
+            while time.perf_counter() < deadline and len(batch) < self.window_max:
                 try:
                     batch.append(self._q.get(timeout=max(deadline - time.perf_counter(), 1e-4)))
                 except queue.Empty:

@@ -275,8 +275,11 @@ int bb_engine_set_recursion_upstreams(bb_engine* e, const uint32_t* ip, const ui
 #define BB_MATCH_MAX_RESPONSES 1048576  /* received datagrams per match call */
 /*
  * bb_forward_batch: miss j = pkts[pkt_off[j] .. pkt_off[j+1]), n <= BB_FORWARD_MAX (and <= max_batch).  For each miss:
- *   route[j]    the index of its datacenter in the filter's list (the pre-filter's suffix and label scan), BB_ROUTE_PTR
- *               for a PTR query, BB_ROUTE_NONE when the upstream table has no upstream for it or the packet does not decode
+ *   route[j]    the index of its datacenter in the filter's list, BB_ROUTE_PTR for a PTR query, BB_ROUTE_NONE when the
+ *               upstream table has no upstream for it or the packet does not decode.  The datacenter is found as
+ *               lib/recursion.js:329-344 finds it in the dotted name, labels joined with '.' and a '.' inside a label
+ *               kept as it is: the name must end with the region domain (compared as bytes), and the datacenter is the
+ *               rest of the name without the character before that suffix, after its last '.'
  *   its upstream query, byte for byte what recursion.py's _exchange sends except the ID: the client's flags & 0x7800
  *               (opcode kept, RD cleared), QDCOUNT 1, no other records, the client's QNAME, QTYPE and QCLASS; no OPT.
  *               ID = F(j), a keyed bijection on 16 bits (4-round Feistel network, round keys from id_key): the IDs of
