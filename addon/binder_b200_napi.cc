@@ -12,6 +12,7 @@
 //   const r = bb.resolveBatch(engine, pkts /*Buffer*/, pktOff /*Uint32Array n+1*/, seed /*BigInt*/);
 //   // r = {out: Buffer, outOff: Uint32Array, outLen: Uint16Array, status: Uint8Array, miss: Uint32Array}
 #include <node_api.h>
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <vector>
@@ -180,6 +181,47 @@ static napi_value RelayBatch(napi_env env, napi_callback_info info) {
     napi_set_named_property(env, res, "out", o_out);   napi_set_named_property(env, res, "outOff", t_oo);
     napi_set_named_property(env, res, "outLen", t_ol); napi_set_named_property(env, res, "status", t_st);
     return res;
+}
+
+// logBatch(engine, out: Buffer, outOff: Uint32Array, outLen: Uint16Array(n), status: Uint8Array(n))
+//   -> {log: Buffer, logOff: Uint32Array(n+1), logLen: Uint32Array(n), headLen: Uint16Array(n), summary: Uint32Array(n)}:
+//   binder's "DNS query" record of each response of a resolveBatch / relayBatch result (bb_log_batch, lib/server.js:509-591).
+//   Record i = log[logOff[i] .. +logLen[i]); its first headLen[i] bytes are the head, the rest the body (DESIGN.md section 15).
+static napi_value LogBatch(napi_env env, napi_callback_info info) {
+    size_t argc = 5; napi_value argv[5];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    if (argc < 5) return Throw(env, BB_ERR_ARG);
+    void* e; NAPI_OK(napi_get_value_external(env, argv[0], &e));
+    void* out; size_t outlen; NAPI_OK(napi_get_buffer_info(env, argv[1], &out, &outlen));
+    napi_typedarray_type t1, t2, t3; size_t n1, n2, n3; void *p1, *p2, *p3; napi_value ab; size_t bo;
+    NAPI_OK(napi_get_typedarray_info(env, argv[2], &t1, &n1, &p1, &ab, &bo));
+    NAPI_OK(napi_get_typedarray_info(env, argv[3], &t2, &n2, &p2, &ab, &bo));
+    NAPI_OK(napi_get_typedarray_info(env, argv[4], &t3, &n3, &p3, &ab, &bo));
+    // the offsets and lengths need not be checked here: the kernel bounds-checks every response against outlen
+    if (t1 != napi_uint32_array || t2 != napi_uint16_array || t3 != napi_uint8_array || n1 < n3 || n2 < n3 || n3 > (1u << 22) ||
+        outlen > 0xFFFFFFFFu)
+        return Throw(env, BB_ERR_ARG);
+    const uint32_t n = (uint32_t)n3;
+    void *lo, *ll, *hl, *sm; napi_value a_lo, a_ll, a_hl, a_sm, t_lo, t_ll, t_hl, t_sm;
+    NAPI_OK(napi_create_arraybuffer(env, ((size_t)n + 1) * 4, &lo, &a_lo)); NAPI_OK(napi_create_typedarray(env, napi_uint32_array, n + 1, a_lo, 0, &t_lo));
+    NAPI_OK(napi_create_arraybuffer(env, (size_t)n * 4, &ll, &a_ll));       NAPI_OK(napi_create_typedarray(env, napi_uint32_array, n, a_ll, 0, &t_ll));
+    NAPI_OK(napi_create_arraybuffer(env, (size_t)n * 2, &hl, &a_hl));       NAPI_OK(napi_create_typedarray(env, napi_uint16_array, n, a_hl, 0, &t_hl));
+    NAPI_OK(napi_create_arraybuffer(env, (size_t)n * 4, &sm, &a_sm));       NAPI_OK(napi_create_typedarray(env, napi_uint32_array, n, a_sm, 0, &t_sm));
+    // a record can be far longer than its response: start at 4 bytes per response byte + 256 per record, grow on overflow
+    uint64_t cap = std::max<uint64_t>(4096, std::min<uint64_t>(4ull * outlen + 256ull * n, 0xFFFFFF00u));
+    for (;;) {
+        void* lg; napi_value b_lg;
+        NAPI_OK(napi_create_buffer(env, (size_t)cap, &lg, &b_lg));
+        int rc = bb_log_batch((bb_engine*)e, (const uint8_t*)out, (uint32_t)outlen, (const uint32_t*)p1, (const uint16_t*)p2,
+                              (const uint8_t*)p3, n, (uint8_t*)lg, (uint32_t)cap, (uint32_t*)lo, (uint32_t*)ll, (uint16_t*)hl, (uint32_t*)sm);
+        if (rc == BB_ERR_CAPACITY && cap < 0xFFFFFF00u) { cap = std::min<uint64_t>(cap * 4, 0xFFFFFF00u); continue; }
+        if (rc != BB_OK) return Throw(env, rc);
+        napi_value res; NAPI_OK(napi_create_object(env, &res));
+        napi_set_named_property(env, res, "log", b_lg);      napi_set_named_property(env, res, "logOff", t_lo);
+        napi_set_named_property(env, res, "logLen", t_ll);   napi_set_named_property(env, res, "headLen", t_hl);
+        napi_set_named_property(env, res, "summary", t_sm);
+        return res;
+    }
 }
 
 // engineSetRecursionUpstreams(engine, ip: Uint32Array, port: Uint16Array, dc: Uint8Array)   (bb_engine_set_recursion_upstreams;
@@ -484,6 +526,7 @@ static napi_value Init(napi_env env, napi_value exports) {
         { "engineSetRecursionFilter", nullptr, EngineSetRecursionFilter, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "resolveBatch", nullptr, ResolveBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "relayBatch", nullptr, RelayBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "logBatch", nullptr, LogBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "engineSetRecursionUpstreams", nullptr, EngineSetRecursionUpstreams, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "forwardBatch", nullptr, ForwardBatch, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "matchUpstreams", nullptr, MatchUpstreams, nullptr, nullptr, nullptr, napi_default, nullptr },

@@ -55,6 +55,10 @@ SYMBOLS = {
     'bb_relay_batch': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p,
                                                       _c.c_void_p]),
     'bb_relay_batch_device': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_uint32, _c.c_uint32, _c.c_void_p, _c.c_uint32] + [_c.c_void_p] * 5),
+    'bb_log_batch': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_uint32] + [_c.c_void_p] * 3 + [_c.c_uint32, _c.c_void_p, _c.c_uint32] +
+                     [_c.c_void_p] * 4),
+    'bb_log_batch_device': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_uint32] + [_c.c_void_p] * 4 + [_c.c_uint32, _c.c_void_p,
+                                                                                                      _c.c_uint32] + [_c.c_void_p] * 6),
     'bb_engine_set_recursion_upstreams': (_c.c_int, [_c.c_void_p] * 4 + [_c.c_uint32]),
     'bb_forward_batch': (_c.c_int, [_c.c_void_p] * 3 + [_c.c_uint32, _c.c_uint64, _c.c_void_p, _c.c_uint32] + [_c.c_void_p] * 4),
     'bb_forward_batch_device': (_c.c_int, [_c.c_void_p] * 5 + [_c.c_uint32, _c.c_uint64, _c.c_void_p, _c.c_uint32] +

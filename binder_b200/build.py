@@ -11,7 +11,8 @@ SO = os.path.join(HERE, 'libbinder_b200.so')
 SRCS = [os.path.join(HERE, 'csrc', f) for f in ('engine.cu', 'zone_build.cpp', 'balancer_frames.cpp', 'balancer_relay.cpp',
                                                 'balancer_tcp.cpp')]
 DEPS = SRCS + [os.path.join(HERE, 'csrc', 'zone_image.h'), os.path.join(HERE, 'csrc', 'resolve_device.cuh'),
-               os.path.join(HERE, 'csrc', 'balancer_backend.h'), os.path.join(HERE, 'csrc', 'relay_device.cuh'), os.path.join(HERE, 'csrc', 'forward_device.cuh'),
+               os.path.join(HERE, 'csrc', 'balancer_backend.h'), os.path.join(HERE, 'csrc', 'relay_device.cuh'), os.path.join(HERE, 'csrc', 'log_device.cuh'),
+               os.path.join(HERE, 'csrc', 'forward_device.cuh'),
                os.path.join(os.path.dirname(HERE), 'include', 'binder_b200.h')]
 NVCC = os.environ.get('NVCC', '/usr/local/cuda/bin/nvcc')
 FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',

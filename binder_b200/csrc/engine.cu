@@ -10,6 +10,8 @@
 //   miss hand-off to recursion        -> compacted miss_idx[]     (lib/server.js:110-113,222-225)
 // and a second kernel turns the upstream responses to forwarded misses into binder's replies:
 //   Recursion.resolve's respond()     -> relay_kernel / relay_size() + relay_emit()   (lib/recursion.js:287-327)
+// and an opt-in third turns a result set into binder's per-query "DNS query" log records:
+//   server.on('after') record         -> log_kernel / log_record()                    (lib/server.js:509-591)
 //
 // Data movement (HBM-bound integer/byte work, no tensor cores):
 //   * a CTA owns a tile of 128 consecutive queries; their packed bytes are one contiguous
@@ -36,6 +38,7 @@ extern "C" uint64_t bb_zone_sync_gen(const bb_zone* z);
 
 #include "resolve_device.cuh"
 #include "relay_device.cuh"
+#include "log_device.cuh"
 #include "forward_device.cuh"
 
 namespace bbk {
@@ -571,6 +574,95 @@ __global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
         });
 }
 
+// ---- query log (DESIGN.md section 15, lib/server.js:509-591) ---------------------------------------------------------
+// One launch per result set.  A CTA takes a tile of 128 responses, a thread per response.  When the tile's responses lie
+// in one range that fits, it is staged into shared memory with one bulk copy (a resolve tile's responses are contiguous
+// in either packing; a caller's result set need not be), otherwise the threads read global memory.  Then the record's
+// sizing pass (log_record), a CTA scan, placement, and the emit pass straight to the output, or through the bounce buffer
+// to pinned host memory as the relay does.  Self-cleaning: a call is one launch.
+constexpr int LS_R = 32768;               // staged response bytes per tile
+struct LogParams {
+    const uint8_t* resp; uint32_t resp_bytes; const uint32_t* resp_totals;
+    const uint32_t* out_off; const uint16_t* out_len; const uint8_t* status; uint32_t n;
+    const EngineConst* eng; uint32_t suffix_len;
+    uint8_t* log; uint32_t log_cap; uint32_t* log_off; uint32_t* log_len; uint16_t* head_len; uint32_t* summary; uint32_t* totals;
+    uint8_t* bounce;                      // zero-copy results: device buffer (same offsets as `log`) written first
+    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap;
+    uint32_t epoch;
+};
+
+template <bool ORDERED>
+__global__ void __launch_bounds__(T) log_kernel(const LogParams P) {
+    __shared__ __align__(16) uint8_t s_r[LS_R + 32];
+    __shared__ uint32_t s_wsum[T / 32], s_lo, s_hi;
+    __shared__ unsigned long long s_prefix;
+    __shared__ __align__(8) unsigned long long s_bar;
+    const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+    const uint32_t tile = blockIdx.x, n = P.n, ntiles = (n + T - 1) / T;
+    if (tile < ntiles) {
+        const uint32_t q0 = tile * T, nq = min((uint32_t)T, n - q0);
+        // the response bytes: the caller's count, or the resolve / relay launch's totals[0] that produced them
+        const uint32_t rb = P.resp_totals ? min(P.resp_totals[0], P.resp_bytes) : P.resp_bytes;
+        if (tid == 0) { s_lo = 0xFFFFFFFFu; s_hi = 0; }
+        __syncthreads();
+        uint32_t o = 0, l = 0;
+        bool answered = false, in = false;
+        if (tid < (int)nq) {
+            answered = P.status[q0 + tid] == ST_ANSWERED;
+            if (answered) {
+                o = P.out_off[q0 + tid]; l = P.out_len[q0 + tid];
+                in = o <= rb && l <= rb - o;                 // outside the response bytes: the bad bit
+                if (in) { atomicMin(&s_lo, o); atomicMax(&s_hi, o + l); }
+            }
+        }
+        __syncthreads();
+        const uint32_t lo = s_lo, hi = s_hi;                 // lo > hi: nothing to read
+        const uint32_t bar = (uint32_t)__cvta_generic_to_shared(&s_bar);
+        if (tid == 0) { mbar_init(bar, 1); stage_range(bar, s_r, P.resp, lo, hi, LS_R); }
+        __syncthreads();
+        const bool staged = stage_wait(bar, lo, hi, LS_R);
+
+        // ---- sizing ----
+        const uint8_t* up = in ? (staged ? s_r + (o - (lo & ~15u)) : P.resp + o) : nullptr;
+        const uint8_t* sfx = P.eng->suffix;
+        uint32_t sum = answered ? LOG_BAD : 0, hl = 0;
+        Txt t{ nullptr, 0 };
+        if (in) sum = log_record(up, l, sfx, P.suffix_len, t, hl);
+        const uint32_t len = (sum & LOG_BAD) ? 0 : t.n;
+        // ---- CTA scan of the record sizes, placement (bytes | records << D_MISS_SHIFT) ----
+        const uint32_t nrec = __syncthreads_count(len != 0);
+        const TileScan sc = cta_scan<false>(len, 0, s_wsum, nullptr, lane, warp);
+        const uint32_t my_o = sc.ex, tile_bytes = sc.tot;
+        const uint64_t gbase = place_tile<ORDERED>(P.desc, P.ntiles_cap, tile, tile_bytes, nrec, s_prefix, tid) & ((1ull << D_MISS_SHIFT) - 1);
+        const bool overflow = gbase + tile_bytes > (uint64_t)P.log_cap;
+        if (tid < (int)nq) {
+            P.log_off[q0 + tid] = (uint32_t)(gbase + my_o);
+            P.log_len[q0 + tid] = len;
+            P.head_len[q0 + tid] = (uint16_t)(len ? hl : 0);
+            if (P.summary) P.summary[q0 + tid] = sum;
+        }
+        if (overflow && tid == 0) P.totals[2] = P.epoch;
+        // ---- emit ----
+        if (!overflow) {
+            uint8_t* const dst = P.bounce ? P.bounce : P.log;
+            if (len) { Txt w{ dst + gbase + my_o, 0 }; log_record(up, l, sfx, P.suffix_len, w, hl); }
+            if (P.bounce && tile_bytes) {                 // the tile's contiguous range to pinned host memory, 16 bytes per store
+                __syncthreads();
+                const uint8_t* src = P.bounce + gbase;
+                flush_range(P.log + gbase, gbase, 0, tile_bytes, [=](uint32_t x, uint32_t k) { return src + x + k; }, tid);
+            }
+        }
+    }
+    // ---- self-cleaning: the last block publishes the totals and resets the placement state ----
+    if (warp == 0)
+        self_clean<ORDERED>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+            const uint64_t tb = cur & ((1ull << D_MISS_SHIFT) - 1);
+            P.log_off[n] = (uint32_t)tb; P.totals[0] = (uint32_t)tb; P.totals[1] = (uint32_t)(cur >> D_MISS_SHIFT);
+            if (tb > P.log_cap) P.totals[2] = P.epoch;
+            P.totals[3] = P.epoch;
+        });
+}
+
 // ---- recursion forward and match (DESIGN.md section 14, lib/recursion.js:253-280,335-354,382-387) ----------------------
 // Forward: three launches per call.  forward_kernel takes a tile of 128 misses, a thread per miss: decode, route, the
 // client query packed in miss order (CTA scan + look-back placement, the relay's input as it stands) and the tile's
@@ -1050,10 +1142,11 @@ struct bb_engine {
     uint32_t* h_fb = nullptr;
     // the zone this engine last synchronised with (incremental updates only continue from that state)
     const bb_zone* zone = nullptr; uint64_t zone_gen = 0; uint64_t arena_cap = 0;
-    // the device staging of bb_relay_batch, bb_forward_batch and bb_match_upstreams (stage): one block for all three, as
-    // they run synchronously on slot 0's stream
+    // the device staging of bb_relay_batch, bb_forward_batch, bb_match_upstreams and bb_log_batch (stage): one block for
+    // all of them, as they run synchronously on slot 0's stream
     uint8_t* staging = nullptr; size_t staging_cap = 0;
     PinnedCheck r_pinned;                        // of bb_relay_batch's output sets
+    PinnedCheck l_pinned;                        // of bb_log_batch's output sets
 };
 
 // A launch's placement scratch: desc[max_tiles] (each tile's published prefix), the arrival cursor in desc[max_tiles], the
@@ -1443,6 +1536,79 @@ int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t*
     if (rc != BB_OK) return rc;
     return relay_launch(e, *c, d_q_pkts, d_q_off, d_up_pkts, d_up_off, n, flags, d_out, out_cap, d_out_off, d_out_len, d_status,
                         d_totals, nullptr);
+}
+
+// ---- query log (lib/server.js:509-591) ------------------------------------------------------------------------------
+static int log_launch(bb_engine* e, const StreamCtx& c, const uint8_t* resp, uint32_t resp_bytes, const uint32_t* resp_totals,
+                      const uint32_t* out_off, const uint16_t* out_len, const uint8_t* status, uint32_t n, uint8_t* log,
+                      uint32_t log_cap, uint32_t* log_off, uint32_t* log_len, uint16_t* head_len, uint32_t* summary,
+                      uint32_t* totals, uint8_t* bounce) {
+    bbk::LogParams P;
+    P.resp = resp; P.resp_bytes = resp_bytes; P.resp_totals = resp_totals; P.out_off = out_off; P.out_len = out_len;
+    P.status = status; P.n = n; P.eng = e->d_const; P.suffix_len = e->hconst.suffix_len;
+    P.log = log; P.log_cap = log_cap; P.log_off = log_off; P.log_len = log_len; P.head_len = head_len; P.summary = summary;
+    P.totals = totals; P.bounce = bounce;
+    place_params(e, c.desc, P);
+    const uint32_t ntiles = (n + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;   // an empty set still reports its totals
+    if (e->ordered) bbk::log_kernel<true><<<grid, bbk::T, 0, c.stream>>>(P);
+    else bbk::log_kernel<false><<<grid, bbk::T, 0, c.stream>>>(P);
+    CK(cudaGetLastError());
+    e->launches++;
+    return BB_OK;
+}
+
+int bb_log_batch(bb_engine* e, const uint8_t* resp, uint32_t resp_bytes, const uint32_t* out_off, const uint16_t* out_len,
+                 const uint8_t* status, uint32_t n, uint8_t* log, uint32_t log_cap, uint32_t* log_off, uint32_t* log_len,
+                 uint16_t* head_len, uint32_t* summary) {
+    if (!e || !log_off || n > e->max_batch) return BB_ERR_ARG;
+    if (n && (!out_off || !out_len || !status || !log || !log_len || !head_len || (resp_bytes && !resp))) return BB_ERR_ARG;
+    CK(cudaSetDevice(e->device));
+    // zero-copy results when every output buffer is pinned host memory, as bb_relay_batch: the device log is then the
+    // kernel's bounce buffer.  Without a summary the log buffer stands in for it, so that the check always covers five.
+    const void* outs[5] = { log, log_off, log_len, head_len, summary ? (const void*)summary : log };
+    const bool zc = e->l_pinned.check(outs, 5) && n != 0;
+    uint8_t *d_resp, *d_status, *d_log; uint32_t *d_totals, *d_off, *d_log_off, *d_log_len, *d_summary; uint16_t *d_len, *d_head_len;
+    int rc = stage(e, { { d_totals, 16 }, { d_resp, (size_t)resp_bytes + 64 }, { d_off, (size_t)n * 4 + 16 }, { d_len, (size_t)n * 2 + 16 },
+                        { d_status, (size_t)n + 16 }, { d_log, (size_t)log_cap + 64 }, { d_log_off, zc ? 0 : ((size_t)n + 1) * 4 },
+                        { d_log_len, zc ? 0 : (size_t)n * 4 + 16 }, { d_head_len, zc ? 0 : (size_t)n * 2 + 16 },
+                        { d_summary, zc || !summary ? 0 : (size_t)n * 4 + 16 } });
+    if (rc != BB_OK) return rc;
+    const StreamCtx& c = e->sync;
+    if (resp_bytes) CK(cudaMemcpyAsync(d_resp, resp, resp_bytes, cudaMemcpyHostToDevice, c.stream));
+    if (n) {
+        CK(cudaMemcpyAsync(d_off, out_off, (size_t)n * 4, cudaMemcpyHostToDevice, c.stream));
+        CK(cudaMemcpyAsync(d_len, out_len, (size_t)n * 2, cudaMemcpyHostToDevice, c.stream));
+        CK(cudaMemcpyAsync(d_status, status, n, cudaMemcpyHostToDevice, c.stream));
+    }
+    rc = log_launch(e, c, d_resp, resp_bytes, nullptr, d_off, d_len, d_status, n, zc ? log : d_log, log_cap, zc ? log_off : d_log_off,
+                    zc ? log_len : d_log_len, zc ? head_len : d_head_len, zc ? summary : summary ? d_summary : nullptr, d_totals,
+                    zc ? d_log : nullptr);
+    if (rc != BB_OK) return rc;
+    const uint32_t epoch = (uint32_t)e->epoch;
+    uint32_t tot[4];
+    CK(cudaMemcpyAsync(tot, d_totals, 16, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
+    if (tot[2] == epoch || tot[0] > log_cap) return BB_ERR_CAPACITY;
+    if (zc) return BB_OK;                        // everything is already in the caller's buffers
+    if (tot[0]) CK(cudaMemcpyAsync(log, d_log, tot[0], cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaMemcpyAsync(log_off, d_log_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
+    if (n) CK(cudaMemcpyAsync(log_len, d_log_len, (size_t)n * 4, cudaMemcpyDeviceToHost, c.stream));
+    if (n) CK(cudaMemcpyAsync(head_len, d_head_len, (size_t)n * 2, cudaMemcpyDeviceToHost, c.stream));
+    if (n && summary) CK(cudaMemcpyAsync(summary, d_summary, (size_t)n * 4, cudaMemcpyDeviceToHost, c.stream));
+    CK(cudaStreamSynchronize(c.stream));
+    return BB_OK;
+}
+
+int bb_log_batch_device(bb_engine* e, const uint8_t* d_resp, uint32_t resp_bytes, const uint32_t* d_resp_totals,
+                        const uint32_t* d_out_off, const uint16_t* d_out_len, const uint8_t* d_status, uint32_t n,
+                        uint8_t* d_log, uint32_t log_cap, uint32_t* d_log_off, uint32_t* d_log_len, uint16_t* d_head_len,
+                        uint32_t* d_summary, uint32_t* d_totals, void* stream) {
+    if (!e || n > e->max_batch || ((uintptr_t)d_resp & 15) || ((uintptr_t)d_log & 15)) return BB_ERR_ARG;
+    StreamCtx* c = nullptr;
+    int rc = stream_ctx(e, stream, &c);
+    if (rc != BB_OK) return rc;
+    return log_launch(e, *c, d_resp, resp_bytes, d_resp_totals, d_out_off, d_out_len, d_status, n, d_log, log_cap, d_log_off,
+                      d_log_len, d_head_len, d_summary, d_totals, nullptr);
 }
 
 // ---- recursion forward and match (lib/recursion.js:253-280,335-354,382-387) --------------------------------------------

@@ -17,7 +17,10 @@ enum { UT_A = 1, UT_CNAME = 5, UT_PTR = 12, UT_TXT = 16, UT_AAAA = 28, UT_SRV = 
 // `end` = first byte after the name's bytes at `pos` (its terminator or its first pointer), `wl` = decompressed wire
 // length with the terminator.  With `w`, the decompressed labels are written out (original case, no compression).
 // Termination: a run of pointers strictly decreases, and every label in between adds to the 255-byte budget.
-__device__ bool up_name(const uint8_t* u, uint32_t len, uint32_t pos, uint32_t& end, uint32_t& wl, Out* w) {
+// W is any sink with u8() (a length byte, 0 for the terminator) and copy() (a label's bytes): the relay writes the labels
+// with Out, the query log (log_device.cuh) renders them as a dotted string.
+template <class W>
+__device__ bool up_name(const uint8_t* u, uint32_t len, uint32_t pos, uint32_t& end, uint32_t& wl, W* w) {
     uint32_t p = pos, n = 0;
     bool jumped = false;
     for (;;) {
@@ -53,7 +56,7 @@ struct UpRR { uint32_t type, klass, ttl, rd, rdlen, nwl; };
 // CNAME, PTR and SRV is valid and ends inside RDLEN.  -> false when malformed; else `pos` moves past the RR.
 __device__ bool up_rr(const uint8_t* u, uint32_t len, uint32_t& pos, UpRR& rr) {
     uint32_t end = 0, wl = 0;
-    if (!up_name(u, len, pos, end, wl, nullptr) || end + 10 > len) return false;
+    if (!up_name<Out>(u, len, pos, end, wl, nullptr) || end + 10 > len) return false;
     rr.type = be16(u + end); rr.klass = be16(u + end + 2);
     rr.ttl = be16(u + end + 4) << 16 | be16(u + end + 6);
     rr.rdlen = be16(u + end + 8); rr.rd = end + 10; rr.nwl = 0;
@@ -62,8 +65,8 @@ __device__ bool up_rr(const uint8_t* u, uint32_t len, uint32_t& pos, UpRR& rr) {
     switch (rr.type) {
     case UT_A: if (rr.rdlen != 4) return false; break;
     case UT_AAAA: if (rr.rdlen != 16) return false; break;
-    case UT_SRV: if (rr.rdlen < 7 || !up_name(u, len, rr.rd + 6, end, rr.nwl, nullptr) || end > rdend) return false; break;
-    case UT_CNAME: case UT_PTR: if (!up_name(u, len, rr.rd, end, rr.nwl, nullptr) || end > rdend) return false; break;
+    case UT_SRV: if (rr.rdlen < 7 || !up_name<Out>(u, len, rr.rd + 6, end, rr.nwl, nullptr) || end > rdend) return false; break;
+    case UT_CNAME: case UT_PTR: if (!up_name<Out>(u, len, rr.rd, end, rr.nwl, nullptr) || end > rdend) return false; break;
     }
     pos = rdend;
     return true;
@@ -104,7 +107,7 @@ __device__ void relay_size(const uint8_t* q, uint32_t qlen, const uint8_t* u, ui
         an = be16(u + 6);
         for (uint32_t i = 0; ok && i < qd; i++) {                 // questions: skipped, but they must be well formed
             uint32_t end = 0, wl = 0;
-            ok = up_name(u, ulen, pos, end, wl, nullptr) && end + 4 <= ulen;
+            ok = up_name<Out>(u, ulen, pos, end, wl, nullptr) && end + 4 <= ulen;
             pos = end + 4;
         }
         R.an0 = pos;

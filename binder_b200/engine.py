@@ -16,6 +16,7 @@ from ._lib import check, lib
 ANSWERED, MISS_RECURSE, DROPPED = 0, 1, 2
 ROUTE_PTR, ROUTE_NONE = 16, 17          # forward routes after the 16 datacenter indices (BB_ROUTE_PTR, BB_ROUTE_NONE)
 FORWARD_ROUTES = 18
+ERR_CAPACITY = -5                       # BB_ERR_CAPACITY
 
 
 def ip_u32(addr):
@@ -191,6 +192,46 @@ class Engine(object):
         """bb_relay_batch_device; pointers are raw device addresses."""
         check(lib().bb_relay_batch_device(self._h, d_q, d_q_off, d_up, d_up_off, n, 1 if tcp else 0, d_out, out_cap, d_out_off,
                                           d_out_len, d_status, d_totals, stream))
+
+    # -- query log (bb_log_batch, lib/server.js:509-591) ---------------------------------------
+    def log_batch(self, out, out_off, out_len, status, summary=False, buffers=None):
+        """binder's "DNS query" log records of a result set (resolve_batch's or relay_batch's out, out_off, out_len,
+        status) -> (log uint8[total], log_off uint32[n+1], log_len uint32[n], head_len uint16[n][, summary uint32[n]]):
+        record i = log[log_off[i] : log_off[i] + log_len[i]], its first head_len[i] bytes the head fragment, the rest the
+        body (DESIGN.md section 15).  buffers: optional (log, log_off, log_len, head_len, summary) to fill, e.g. pinned
+        ones from bb_host_alloc (then returned as views; summary may be None)."""
+        out = np.ascontiguousarray(out, dtype=np.uint8)
+        out_off = np.ascontiguousarray(out_off, dtype=np.uint32)
+        out_len = np.ascontiguousarray(out_len, dtype=np.uint16)
+        status = np.ascontiguousarray(status, dtype=np.uint8)
+        n = len(status)
+        if len(out_off) < n or len(out_len) < n:
+            raise ValueError('one offset and one length per status')
+        fixed = buffers is not None
+        if fixed and summary and buffers[4] is None:
+            raise ValueError('summary=True needs a summary buffer in buffers')
+        cap = len(buffers[0]) if fixed else max(4096, min(4 * len(out) + 256 * n, 0xFFFFFF00))
+        while True:
+            if not fixed:
+                buffers = (np.empty(cap, dtype=np.uint8), np.zeros(n + 1, dtype=np.uint32), np.zeros(max(n, 1), dtype=np.uint32),
+                           np.zeros(max(n, 1), dtype=np.uint16), np.zeros(max(n, 1), dtype=np.uint32) if summary else None)
+            log, log_off, log_len, head_len, summ = buffers
+            rc = lib().bb_log_batch(self._h, out.ctypes.data, len(out), out_off.ctypes.data, out_len.ctypes.data,
+                                    status.ctypes.data, n, log.ctypes.data, len(log), log_off.ctypes.data, log_len.ctypes.data,
+                                    head_len.ctypes.data, summ.ctypes.data if summ is not None else None)
+            if rc == ERR_CAPACITY and not fixed and cap < 0xFFFFFF00:
+                cap = min(cap * 4, 0xFFFFFF00)               # a record can be far longer than its response: try again
+                continue
+            check(rc)
+            break
+        res = (log[:log_off[n]].copy(), log_off[:n + 1], log_len[:n], head_len[:n])
+        return res + (summ[:n],) if summary else res
+
+    def log_device(self, d_resp, resp_bytes, d_resp_totals, d_out_off, d_out_len, d_status, n, d_log, log_cap, d_log_off,
+                   d_log_len, d_head_len, d_summary, d_totals, stream=0):
+        """bb_log_batch_device; pointers are raw device addresses (d_resp_totals and d_summary may be 0)."""
+        check(lib().bb_log_batch_device(self._h, d_resp, resp_bytes, d_resp_totals or None, d_out_off, d_out_len, d_status, n, d_log,
+                                        log_cap, d_log_off, d_log_len, d_head_len, d_summary or None, d_totals, stream))
 
     # -- recursion forward and match (bb_forward_batch, bb_match_upstreams, lib/recursion.js:253-280,335-354,382-387) --
     def set_recursion_upstreams(self, upstreams):

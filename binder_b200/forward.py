@@ -60,12 +60,17 @@ class GpuRecursion(object):
         self._thread = threading.Thread(target=self._loop, daemon=True)
         self._thread.start()
 
-    def resolve(self, packet, addr, sock):
-        """options.recursion.resolve(query, cb) (lib/server.js:110-113,222-225) for one miss."""
+    def resolve(self, packet, addr, sock, received=None):
+        """options.recursion.resolve(query, cb) (lib/server.js:110-113,222-225) for one miss.  received: when the query
+        arrived (time.time(); default now), the start of its query log line's latency."""
         if addr is None:
             self.counters['tcp_skipped'] += 1
             return
-        self._q.put((bytes(packet), self._udp, (addr, sock)))
+        self._q.put((bytes(packet), self._udp, (addr, sock, time.time() if received is None else received)))
+
+    def set_query_log(self, query_log):
+        """The server's query log sink (binder_b200.query_log.QueryLog): relayed UDP replies get their lines too."""
+        self._udp.query_log = query_log
 
     def submit(self, packet, sink, tag):
         """One miss of a transport owner: its upstream response comes back through sink.relay(..., tags) with `tag`."""

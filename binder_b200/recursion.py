@@ -74,10 +74,11 @@ class QueueSink(object):
 
 class UdpSink(object):
     """resolve()'s delivery: the window's UDP misses relayed as one batch on `resolver`, each reply sent from the
-    listener's socket to the client; the tag is (addr, sock).  A failed relay batch gets no replies and is counted."""
+    listener's socket to the client; the tag is (addr, sock, when the query arrived).  A failed relay batch gets no replies and is counted."""
 
     def __init__(self, resolver, counters):
         self.resolver, self.counters = resolver, counters
+        self.query_log = None             # binder_b200.query_log.QueryLog: a line per reply sent (the server's sink)
 
     def relay(self, q_data, q_off, up, up_off, tags):
         try:
@@ -85,13 +86,15 @@ class UdpSink(object):
         except Exception:                 # BinderError (capacity, CUDA): this window gets no replies
             self.counters['failed_batches'] += 1
             return
-        for i, (addr, sock) in enumerate(tags):
+        for i, (addr, sock, _) in enumerate(tags):
             if status[i] == 0:
                 try:
                     sock.sendto(out[out_off[i]:out_off[i] + out_len[i]].tobytes(), addr)
                     self.counters['relayed'] += 1
                 except OSError:
                     pass
+        if self.query_log is not None:
+            self.query_log.write(self.resolver, out, out_off, out_len, status, [t[0] for t in tags], [t[2] for t in tags])
 
 
 def deliver(batch, q_data, q_off, up, up_off, counters):
@@ -145,12 +148,17 @@ class Recursion(object):
             ups = [a for addrs in self.dcs.values() for a in addrs]
         return [a for a in ups if a[0] not in self.my_addrs]
 
-    def resolve(self, packet, addr, sock):
-        """options.recursion.resolve(query, cb) (lib/server.js:110-113,222-225) for one miss."""
+    def resolve(self, packet, addr, sock, received=None):
+        """options.recursion.resolve(query, cb) (lib/server.js:110-113,222-225) for one miss.  received: when the query
+        arrived (time.time(); default now), the start of its query log line's latency."""
         if addr is None:
             self.counters['tcp_skipped'] += 1
             return
-        self._q.put((bytes(packet), self._udp, (addr, sock)))
+        self._q.put((bytes(packet), self._udp, (addr, sock, time.time() if received is None else received)))
+
+    def set_query_log(self, query_log):
+        """The server's query log sink (binder_b200.query_log.QueryLog): relayed UDP replies get their lines too."""
+        self._udp.query_log = query_log
 
     def submit(self, packet, sink, tag):
         """One miss of a transport owner: its reply comes back through sink.relay(..., tags) with `tag`."""

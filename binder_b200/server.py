@@ -17,6 +17,11 @@ connection, length-prefixed.  Relayed replies may overtake local answers on the 
 ID matches them).  A connection owed a relay stays open through the idle sweep and after a half-close until the reply
 is written.
 
+Query log (lib/server.js:509-591): with options['query_log'], a writable binary stream, every batch the server answers
+gets one resolver.log_batch call (bb_log_batch) and every answered query one bunyan "DNS query" line on the stream
+(binder_b200/query_log.py; the request id is the DNS ID).  The same sink goes to the recursion (set_query_log), so that
+relayed replies are logged on both transports when they are sent.  Without the option nothing changes.
+
 The resolver is injected, so the CPU-only plumbing test (BASELINE config 1) drives this same code
 with the CPU oracle, while production passes an Engine.
 """
@@ -100,6 +105,12 @@ class Server(object):
         self._thread = None
         self._stop = threading.Event()
         self._seed = options.get('shuffle_seed', int(time.time() * 1e6))
+        self.query_log = None
+        if options.get('query_log') is not None:
+            from .query_log import QueryLog
+            self.query_log = QueryLog(options['query_log'])
+            if hasattr(self.recursion, 'set_query_log'):
+                self.recursion.set_query_log(self.query_log)
 
     # lib/server.js:609-653: UDP and TCP on the same port (the balancer socket stays host JS)
     def start(self, callback=None):
@@ -143,12 +154,12 @@ class Server(object):
                 continue
             except OSError:
                 break
-            batch = [(pkt, addr)]
+            batch = [(pkt, addr, time.time())]
             deadline = time.perf_counter() + self.window_s
             self._sock.settimeout(max(self.window_s, 1e-4))
             while len(batch) < self.max_batch and time.perf_counter() < deadline:
                 try:
-                    batch.append(self._sock.recvfrom(MAX_UDP + 1))
+                    batch.append(self._sock.recvfrom(MAX_UDP + 1) + (time.time(),))
                 except (socket.timeout, BlockingIOError):
                     break
             self._sock.settimeout(0.05)
@@ -272,8 +283,9 @@ class Server(object):
                     if chunk:
                         c.last = now
                         msgs = c.framer.feed(chunk)
+                        t_recv = time.time()
                         for m in msgs:
-                            pending.append((m, s))
+                            pending.append((m, s, t_recv))
                         c.waiting += len(msgs)
                         if msgs and deadline is None:
                             deadline = now + self.window_s
@@ -283,7 +295,7 @@ class Server(object):
                     want(s)
             if pending and (len(pending) >= self.max_batch or time.perf_counter() >= deadline):
                 self._resolve_and_send_tcp(pending, conns, sink)
-                for s in set(ps for _, ps in pending):
+                for s in set(ps for _, ps, _ in pending):
                     if s in conns:
                         want(s)
                 pending, deadline = [], None
@@ -309,7 +321,7 @@ class Server(object):
                 self.counters['failed_batches'] += 1
                 res = None
         live = set()
-        for i, s in enumerate(tags):
+        for i, (s, _) in enumerate(tags):
             c = conns.get(s)
             if c is None:                            # closed meanwhile
                 continue
@@ -319,41 +331,58 @@ class Server(object):
                 out, out_off, out_len, _ = res
                 c.outq += TcpFramer.frame(out[out_off[i]:out_off[i] + out_len[i]].tobytes())
                 self.counters['tcp_relayed'] += 1
+        if res is not None and self.query_log is not None:
+            self._log(res[:4], [self._peer(s) for s, _ in tags], [t for _, t in tags])
         return live
 
+    @staticmethod
+    def _peer(s):
+        try:
+            return s.getpeername()[:2]
+        except OSError:                              # closed meanwhile: its line still names the query
+            return ('', 0)
+
+    def _log(self, res, clients, received):
+        """The query log lines of one batch of sent responses (resolver calls are serialised, as in _resolve)."""
+        with self._lock:
+            self.query_log.write(self.resolver, *res, clients, received)
+
     def _resolve_and_send_tcp(self, pending, conns, sink=None):
-        pkts = [m for m, _ in pending]
+        pkts = [m for m, _, _ in pending]
         data, off = pack_packets(pkts)
         res = self._resolve(data, off, tcp=True)
         c = self.counters
         c['tcp_batches'] += 1
         c['tcp_queries'] += len(pkts)
-        for _, s in pending:
+        for _, s, _ in pending:
             if s in conns:
                 conns[s].waiting -= 1
         if res is None:
             return
         out, out_off, out_len, status, miss = res
-        for i, (_, s) in enumerate(pending):         # per connection, in arrival order
+        for i, (_, s, _) in enumerate(pending):      # per connection, in arrival order
             if status[i] == 0:
                 if s in conns:
                     conns[s].outq += TcpFramer.frame(out[out_off[i]:out_off[i] + out_len[i]].tobytes())
                 c['answered'] += 1
             elif status[i] == 2:
                 c['dropped'] += 1
+        if self.query_log is not None:
+            self._log((out, out_off, out_len, status), [self._peer(s) for _, s, _ in pending], [t for _, _, t in pending])
         for i in miss:
             c['missed'] += 1
-            s = pending[int(i)][1]
+            _, s, t_recv = pending[int(i)]
             if sink is not None:
                 if s in conns:
                     conns[s].waiting += 1
-                    self.recursion.submit(pkts[int(i)], sink, s)
+                    self.recursion.submit(pkts[int(i)], sink, (s, t_recv))
             elif self.recursion is not None:
                 self.recursion.resolve(pkts[int(i)], None, s)
 
     def _resolve_and_send(self, batch):
-        pkts = [p for p, _ in batch if len(p) <= MAX_UDP]
-        addrs = [a for p, a in batch if len(p) <= MAX_UDP]
+        pkts = [p for p, _, _ in batch if len(p) <= MAX_UDP]
+        addrs = [a for p, a, _ in batch if len(p) <= MAX_UDP]
+        received = [t for p, _, t in batch if len(p) <= MAX_UDP]
         data, off = pack_packets(pkts)
         res = self._resolve(data, off)
         c = self.counters
@@ -368,10 +397,15 @@ class Server(object):
                 c['answered'] += 1
             elif status[i] == 2:
                 c['dropped'] += 1
+        if self.query_log is not None:
+            self._log((out, out_off, out_len, status), addrs, received)
         for i in miss:
             c['missed'] += 1
             if self.recursion is not None:
-                self.recursion.resolve(pkts[int(i)], addrs[int(i)], self._sock)
+                if self.query_log is not None and hasattr(self.recursion, 'set_query_log'):
+                    self.recursion.resolve(pkts[int(i)], addrs[int(i)], self._sock, received=received[int(i)])
+                else:
+                    self.recursion.resolve(pkts[int(i)], addrs[int(i)], self._sock)
 
 
 def createServer(options):

@@ -256,6 +256,36 @@ int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t*
                           const uint32_t* d_up_off, uint32_t n, uint32_t flags, uint8_t* d_out, uint32_t out_cap, uint32_t* d_out_off,
                           uint16_t* d_out_len, uint8_t* d_status, uint32_t* d_totals, void* stream);
 
+/* ---- query log (lib/server.js:509-591, DESIGN.md section 15) ----------------------------------------------------------
+ * bb_log_batch: binder's per-query "DNS query" log record of every response of a result set, the output of
+ * bb_resolve_batch* (either packing, UDP or TCP) or bb_relay_batch*: response i = resp[out_off[i] .. +out_len[i]) with
+ * status[i].  An answered response gets a record of two fragments, the parts of bunyan's line the response decides:
+ *   head   "query":{"name":N,"type":T},"edns":true|false
+ *   body   "rcode":R,"answers":[...],"additional":[...]
+ * Record i = log[log_off[i] .. log_off[i] + log_len[i]), its first head_len[i] bytes the head; log_off[n] = the total.
+ * A miss or a dropped query has no record.  The response bytes are untrusted: every read is bounds-checked, and a
+ * response that does not decode (or lies outside resp_bytes) gets an empty record and the bad bit of its summary.
+ *   summary[i] (may be NULL): qtype | rcode << 16 | edns << 20 | tc << 21 | bad << 22; 0 without a record
+ * BB_ERR_ARG for n > max_batch; BB_ERR_CAPACITY when the records do not fit log_cap.  When log, log_off, log_len,
+ * head_len and summary are all pinned host memory (bb_host_alloc) the kernel writes the results into them directly.
+ * Synchronous.
+ */
+int bb_log_batch(bb_engine* e, const uint8_t* resp, uint32_t resp_bytes, const uint32_t* out_off, const uint16_t* out_len,
+                 const uint8_t* status, uint32_t n, uint8_t* log, uint32_t log_cap, uint32_t* log_off /* n+1 */,
+                 uint32_t* log_len, uint16_t* head_len, uint32_t* summary /* may be NULL */);
+/*
+ * Device-resident form of bb_log_batch, with the contract of bb_resolve_batch_device: d_resp and d_log 16-byte aligned,
+ * d_resp readable up to the next multiple of 16 past its last response; d_totals[4] = {log bytes, records, overflow
+ * marker, done marker}, the markers equal to bb_engine_launch_epoch() of this call when set; up to 16 streams (shared
+ * with bb_resolve_batch_device).  With d_resp_totals (a resolve or relay launch's d_totals, on the same stream) the
+ * response byte count is d_resp_totals[0], read on the device, bounded by resp_bytes: a resolve -> log chain needs no
+ * host round trip.  Asynchronous.
+ */
+int bb_log_batch_device(bb_engine* e, const uint8_t* d_resp, uint32_t resp_bytes, const uint32_t* d_resp_totals,
+                        const uint32_t* d_out_off, const uint16_t* d_out_len, const uint8_t* d_status, uint32_t n,
+                        uint8_t* d_log, uint32_t log_cap, uint32_t* d_log_off, uint32_t* d_log_len, uint16_t* d_head_len,
+                        uint32_t* d_summary, uint32_t* d_totals, void* stream);
+
 /*
  * Recursion forward: the upstream queries of a batch of misses, grouped by datacenter, and the matching of the upstream
  * responses to them.  Replaces Recursion.prototype.resolve's lookup (lib/recursion.js:253-280,335-354,382-387) up to the
