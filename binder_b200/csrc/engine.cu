@@ -164,13 +164,13 @@ __device__ __forceinline__ TileScan cta_scan(uint32_t v, uint32_t v2, uint32_t* 
 // desc[ntiles_cap]; it never waits.  ORDERED: the look-back (warp 0).  The result is published through s_prefix; every
 // thread of the block calls it.
 template <bool ORDERED>
-__device__ __forceinline__ uint64_t place_tile(unsigned long long* desc, uint32_t ntiles_cap, uint32_t tile, uint32_t bytes, uint32_t misses,
+__device__ __forceinline__ uint64_t place_tile(const Place& pl, uint32_t tile, uint32_t bytes, uint32_t misses,
                                                unsigned long long& s_prefix, int tid) {
     const int lane = tid & 31, warp = tid >> 5;
     if (!ORDERED) {
-        if (tid == 0) s_prefix = atomicAdd(desc + ntiles_cap, (unsigned long long)bytes | ((unsigned long long)misses << D_MISS_SHIFT));
+        if (tid == 0) s_prefix = atomicAdd(pl.desc + pl.ntiles_cap, (unsigned long long)bytes | ((unsigned long long)misses << D_MISS_SHIFT));
     } else if (warp == 0) {
-        const uint64_t ex = lookback(desc, tile, (uint64_t)bytes | ((uint64_t)misses << D_MISS_SHIFT), lane);
+        const uint64_t ex = lookback(pl.desc, tile, (uint64_t)bytes | ((uint64_t)misses << D_MISS_SHIFT), lane);
         if (lane == 0) s_prefix = ex;
     }
     __syncthreads();
@@ -194,12 +194,25 @@ __device__ __forceinline__ void flush_range(uint8_t* g, uint64_t ga, uint32_t x0
     if (x0 + tid < x1) g[x0 + tid] = *at(x0 + tid, 0);
 }
 
+// Pinned results: the tile's responses were emitted into the device bounce buffer at the offsets they have in `out`;
+// their contiguous range [gbase, gbase + bytes) moves to `out` (pinned host memory) with coalesced 16-byte stores, as
+// 4-byte stores over PCIe would be ruinous (the bytes are still in L2).  Every thread of the block calls it.
+__device__ __forceinline__ void flush_bounce(uint8_t* out, const uint8_t* bounce, uint64_t gbase, uint32_t bytes, int tid) {
+    if (bounce && bytes) {
+        __syncthreads();
+        const uint8_t* src = bounce + gbase;
+        flush_range(out + gbase, gbase, 0, bytes, [=](uint32_t x, uint32_t k) { return src + x + k; }, tid);
+    }
+}
+
 // Self-cleaning, run by warp 0 of every block (blocks beyond the tiles only take part in the count): the last block to
 // finish reads the final descriptor — the inclusive prefix of the last tile, or the arrival cursor — hands it to
 // publish() in lane 0 (the kernel's totals), and resets the placement state for the next launch.
 template <bool ORDERED, class Publish>
-__device__ __forceinline__ void self_clean(unsigned long long* desc, uint32_t* counter, uint32_t ntiles, uint32_t ntiles_cap,
-                                           int lane, Publish publish) {
+__device__ __forceinline__ void self_clean(const Place& pl, uint32_t ntiles, int lane, Publish publish) {
+    unsigned long long* const desc = pl.desc;
+    const uint32_t ntiles_cap = pl.ntiles_cap;
+    uint32_t* const counter = (uint32_t*)(desc + ntiles_cap + 1);
     uint32_t last = 0;
     // ORDERED: this tile's descriptor store must be visible before it counts itself done.  Arrival
     // packing needs no fence here: the claim was an atomic whose return value this thread already
@@ -266,8 +279,8 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     uint8_t* const r_status = MULTI ? P.status + ry * P.status_stride : P.status;
     uint32_t* const r_miss_idx = MULTI ? (uint32_t*)((uint8_t*)P.miss_idx + ry * P.miss_stride) : P.miss_idx;
     uint32_t* const r_totals = MULTI ? (uint32_t*)((uint8_t*)P.totals + ry * P.totals_stride) : P.totals;
-    unsigned long long* const r_desc = MULTI ? (unsigned long long*)((uint8_t*)P.desc + ry * P.desc_stride) : P.desc;
-    uint32_t* const r_counter = MULTI ? (uint32_t*)((uint8_t*)P.counter + ry * P.desc_stride) : P.counter;
+    const Place r_place = { MULTI ? (unsigned long long*)((uint8_t*)P.place.desc + ry * P.desc_stride) : P.place.desc,
+                            P.place.ntiles_cap, P.place.epoch };
     uint32_t* const r_qidx_out = (MULTI && P.qidx_out) ? (uint32_t*)((uint8_t*)P.qidx_out + ry * P.off_stride) : nullptr;
     uint8_t* const r_bounce = (MULTI && P.bounce) ? P.bounce + ry * P.out_stride : P.bounce;
 
@@ -358,7 +371,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
 
     STAMP(7);
     // ---- where this tile's responses (and misses) go: descriptors and the claim carry bytes | misses << 40 ------------
-    const uint64_t ex = place_tile<ORDERED>(r_desc, P.ntiles_cap, tile, tile_bytes, tile_miss, s_prefix, tid);
+    const uint64_t ex = place_tile<ORDERED>(r_place, tile, tile_bytes, tile_miss, s_prefix, tid);
     STAMP(8);
     const uint64_t gbase = ex & ((1ull << D_MISS_SHIFT) - 1);
     const uint32_t mbase = (uint32_t)(ex >> D_MISS_SHIFT);
@@ -372,7 +385,7 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
         if (my_miss) r_miss_idx[mbase + my_mrank] = q0 + qi;
         if (MULTI && r_qidx_out) r_qidx_out[q0 + qi] = qidx;
     }
-    if (overflow && tid == 0) r_totals[2] = P.epoch;
+    if (overflow && tid == 0) r_totals[2] = P.place.epoch;
 
     // ---- emit ---------------------------------------------------------------------------------------
     // Responses are assembled in (swizzled) shared memory and flushed with aligned 16-byte stores: scattered 4-byte stores
@@ -392,20 +405,14 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     const bool odd_emit = my_len && (!(r.sp && !r.trunc) || my_len > (uint32_t)MAXRESP);
     const bool direct = __syncthreads_or(odd_emit) || (!SVC && tile_bytes > (uint32_t)WIN);
     if (!overflow && direct) {
-        // `out` may be pinned host memory (zero-copy results): 4-byte stores over PCIe would be ruinous,
-        // so such tiles assemble in the device bounce buffer and then move their contiguous range with
-        // coalesced 16-byte stores (the bytes are still in L2)
+        // `out` may be pinned host memory (zero-copy results): such tiles assemble in the bounce buffer (flush_bounce)
         uint8_t* const dst = r_bounce ? r_bounce : r_out;
         if (my_len) {
             if (!(r.sp && !r.trunc)) emit_response(P, r, dst + gbase + my_o, qidx);
             else { WrT<2> w; w.begin_global(dst, (uint32_t)(gbase + my_o)); emit_fast(P, r, w, qidx); }
         }
         STAMP(9);
-        if (r_bounce && tile_bytes) {
-            __syncthreads();
-            const uint8_t* src = r_bounce + gbase;
-            flush_range(r_out + gbase, gbase, 0, tile_bytes, [=](uint32_t x, uint32_t k) { return src + x + k; }, tid);
-        }
+        flush_bounce(r_out, r_bounce, gbase, tile_bytes, tid);
     } else if (!overflow && SVC && tile_bytes > (uint32_t)WIN) {
         const uint32_t s_out_a = (uint32_t)__cvta_generic_to_shared(s_out);
         const uint32_t nr = (tile_bytes + WIN - 1) / WIN;                     // <= NROUNDS
@@ -476,11 +483,11 @@ __global__ void __launch_bounds__(T, SVC ? BB_MIN_BLOCKS - 1 : BB_MIN_BLOCKS) re
     }   // tile < ntiles
     // ---- self-cleaning: the last block to finish publishes the totals and resets the placement state ----------------
     if (warp == 0)
-        self_clean<ORDERED>(r_desc, r_counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+        self_clean<ORDERED>(r_place, ntiles, lane, [&](unsigned long long cur) {
             const uint32_t tb = (uint32_t)(cur & ((1ull << D_MISS_SHIFT) - 1));
-            r_out_off[n] = tb; r_totals[0] = tb; r_totals[1] = (uint32_t)(cur >> D_MISS_SHIFT); r_totals[3] = P.epoch;
+            r_out_off[n] = tb; r_totals[0] = tb; r_totals[1] = (uint32_t)(cur >> D_MISS_SHIFT); r_totals[3] = P.place.epoch;
             // one 16-byte store (one PCIe write, no fence, nothing waits for it): what the host picks the next batch's variant from
-            if (!MULTI && P.fb) *(uint4*)P.fb = make_uint4(tb, n, 0u, P.epoch);
+            if (!MULTI && P.fb) *(uint4*)P.fb = make_uint4(tb, n, 0u, P.place.epoch);
             if (MULTI) {                   // what a host reading only the totals needs to know about the region
                 r_totals[4] = n; r_totals[5] = r_n_dev ? r_n_dev[3] : 0u; r_totals[6] = P.err_in ? *(volatile const uint32_t*)P.err_in : 0u;
             }
@@ -500,8 +507,7 @@ struct RelayParams {
     const uint8_t* q; const uint32_t* q_off; const uint8_t* up; const uint32_t* up_off; uint32_t n;
     uint8_t* out; uint32_t out_cap; uint32_t* out_off; uint16_t* out_len; uint8_t* status; uint32_t* totals;
     uint8_t* bounce;                      // zero-copy results: device buffer (same offsets as `out`) written first
-    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap;
-    uint32_t epoch, tcp;
+    Place place; uint32_t tcp;
 };
 
 template <bool ORDERED>
@@ -547,30 +553,26 @@ __global__ void __launch_bounds__(T) relay_kernel(const RelayParams P) {
         const TileScan sc = cta_scan<false>(R.rlen, 0, s_wsum, nullptr, lane, warp);
         const uint32_t my_o = sc.ex, tile_bytes = sc.tot;
         // ---- placement ----
-        const uint64_t gbase = place_tile<ORDERED>(P.desc, P.ntiles_cap, tile, tile_bytes, 0, s_prefix, tid) & D_VAL;
+        const uint64_t gbase = place_tile<ORDERED>(P.place, tile, tile_bytes, 0, s_prefix, tid) & D_VAL;
         const bool overflow = gbase + tile_bytes > (uint64_t)P.out_cap;
         if (tid < (int)nq) {
             P.out_off[q0 + tid] = (uint32_t)(gbase + my_o);
             P.out_len[q0 + tid] = (uint16_t)R.rlen;
             P.status[q0 + tid] = (uint8_t)R.status;
         }
-        if (overflow && tid == 0) P.totals[2] = P.epoch;
+        if (overflow && tid == 0) P.totals[2] = P.place.epoch;
         // ---- emit ----
         if (!overflow) {
             uint8_t* const dst = P.bounce ? P.bounce : P.out;
             if (R.rlen) relay_emit(qp, upp, ul, R, dst + gbase + my_o);
-            if (P.bounce && tile_bytes) {                 // the tile's contiguous range to pinned host memory, 16 bytes per store
-                __syncthreads();
-                const uint8_t* src = P.bounce + gbase;
-                flush_range(P.out + gbase, gbase, 0, tile_bytes, [=](uint32_t x, uint32_t k) { return src + x + k; }, tid);
-            }
+            flush_bounce(P.out, P.bounce, gbase, tile_bytes, tid);
         }
     }
     // ---- self-cleaning: the last block publishes the totals and resets the placement state ----
     if (warp == 0)
-        self_clean<ORDERED>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+        self_clean<ORDERED>(P.place, ntiles, lane, [&](unsigned long long cur) {
             const uint32_t tb = (uint32_t)cur;
-            P.out_off[n] = tb; P.totals[0] = tb; P.totals[1] = 0; P.totals[3] = P.epoch;
+            P.out_off[n] = tb; P.totals[0] = tb; P.totals[1] = 0; P.totals[3] = P.place.epoch;
         });
 }
 
@@ -587,8 +589,7 @@ struct LogParams {
     const EngineConst* eng; uint32_t suffix_len;
     uint8_t* log; uint32_t log_cap; uint32_t* log_off; uint32_t* log_len; uint16_t* head_len; uint32_t* summary; uint32_t* totals;
     uint8_t* bounce;                      // zero-copy results: device buffer (same offsets as `log`) written first
-    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap;
-    uint32_t epoch;
+    Place place;
 };
 
 template <bool ORDERED>
@@ -633,7 +634,7 @@ __global__ void __launch_bounds__(T) log_kernel(const LogParams P) {
         const uint32_t nrec = __syncthreads_count(len != 0);
         const TileScan sc = cta_scan<false>(len, 0, s_wsum, nullptr, lane, warp);
         const uint32_t my_o = sc.ex, tile_bytes = sc.tot;
-        const uint64_t gbase = place_tile<ORDERED>(P.desc, P.ntiles_cap, tile, tile_bytes, nrec, s_prefix, tid) & ((1ull << D_MISS_SHIFT) - 1);
+        const uint64_t gbase = place_tile<ORDERED>(P.place, tile, tile_bytes, nrec, s_prefix, tid) & ((1ull << D_MISS_SHIFT) - 1);
         const bool overflow = gbase + tile_bytes > (uint64_t)P.log_cap;
         if (tid < (int)nq) {
             P.log_off[q0 + tid] = (uint32_t)(gbase + my_o);
@@ -641,25 +642,21 @@ __global__ void __launch_bounds__(T) log_kernel(const LogParams P) {
             P.head_len[q0 + tid] = (uint16_t)(len ? hl : 0);
             if (P.summary) P.summary[q0 + tid] = sum;
         }
-        if (overflow && tid == 0) P.totals[2] = P.epoch;
+        if (overflow && tid == 0) P.totals[2] = P.place.epoch;
         // ---- emit ----
         if (!overflow) {
             uint8_t* const dst = P.bounce ? P.bounce : P.log;
             if (len) { Txt w{ dst + gbase + my_o, 0 }; log_record(up, l, sfx, P.suffix_len, w, hl); }
-            if (P.bounce && tile_bytes) {                 // the tile's contiguous range to pinned host memory, 16 bytes per store
-                __syncthreads();
-                const uint8_t* src = P.bounce + gbase;
-                flush_range(P.log + gbase, gbase, 0, tile_bytes, [=](uint32_t x, uint32_t k) { return src + x + k; }, tid);
-            }
+            flush_bounce(P.log, P.bounce, gbase, tile_bytes, tid);
         }
     }
     // ---- self-cleaning: the last block publishes the totals and resets the placement state ----
     if (warp == 0)
-        self_clean<ORDERED>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+        self_clean<ORDERED>(P.place, ntiles, lane, [&](unsigned long long cur) {
             const uint64_t tb = cur & ((1ull << D_MISS_SHIFT) - 1);
             P.log_off[n] = (uint32_t)tb; P.totals[0] = (uint32_t)tb; P.totals[1] = (uint32_t)(cur >> D_MISS_SHIFT);
-            if (tb > P.log_cap) P.totals[2] = P.epoch;
-            P.totals[3] = P.epoch;
+            if (tb > P.log_cap) P.totals[2] = P.place.epoch;
+            P.totals[3] = P.place.epoch;
         });
 }
 
@@ -683,7 +680,7 @@ struct FwdParams {
     uint32_t* totals;                     // {upstream bytes, n, error marker, done marker, client bytes}
     unsigned long long* hist;             // [tile][route]: count << 32 | bytes, then the (tile, route) output base
     uint16_t* ulen;                       // [j]: upstream query length
-    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap, epoch;
+    Place place;
 };
 template <class PP>
 __device__ __forceinline__ uint32_t fwd_count(const PP& P, bool& bad) {
@@ -725,21 +722,21 @@ __global__ void __launch_bounds__(T) forward_kernel(const FwdParams P) {
         }
         if (tid < (int)nq) { atomicAdd(&s_cnt[rt], 1u); atomicAdd(&s_byt[rt], ul); }
         const TileScan sc = cta_scan<false>(clen, 0, s_wsum, nullptr, lane, warp);      // 128 x 65,535 < 2^24
-        const uint64_t base = place_tile<true>(P.desc, P.ntiles_cap, tile, sc.tot, 0, s_prefix, tid) & D_VAL;
+        const uint64_t base = place_tile<true>(P.place, tile, sc.tot, 0, s_prefix, tid) & D_VAL;
         const bool ovf = base + sc.tot > (uint64_t)P.q_cap;
         if (tid < (int)nq) {
             const uint32_t at = (uint32_t)(base + sc.ex);
             P.q_off[j] = at; P.route[j] = (uint8_t)rt; P.ulen[j] = (uint16_t)ul;
             if (!ovf) for (uint32_t i = 0; i < clen; i++) P.q[at + i] = pk[i];
         }
-        if (ovf && tid == 0) P.totals[2] = P.epoch;
+        if (ovf && tid == 0) P.totals[2] = P.place.epoch;
         if (tid < (int)NROUTE) P.hist[(size_t)tile * NROUTE + tid] = (unsigned long long)s_cnt[tid] << 32 | s_byt[tid];
     }
     if (warp == 0)
-        self_clean<true>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+        self_clean<true>(P.place, ntiles, lane, [&](unsigned long long cur) {
             const uint32_t tb = (uint32_t)cur;
             P.q_off[n] = tb; P.totals[4] = tb; P.totals[1] = n;
-            if (bad) P.totals[2] = P.epoch;
+            if (bad) P.totals[2] = P.place.epoch;
         });
 }
 
@@ -784,8 +781,8 @@ __global__ void __launch_bounds__(FG_T) forward_group_kernel(const FwdParams P) 
     if (t == 0) {
         const uint32_t tb = (uint32_t)s_rbase[NROUTE];
         P.uq_off[n] = tb; P.totals[0] = tb;
-        if (tb > P.uq_cap) P.totals[2] = P.epoch;
-        P.totals[3] = P.epoch;
+        if (tb > P.uq_cap) P.totals[2] = P.place.epoch;
+        P.totals[3] = P.place.epoch;
     }
 }
 
@@ -796,7 +793,7 @@ __global__ void __launch_bounds__(T) forward_scatter_kernel(const FwdParams P) {
     const int tid = threadIdx.x;
     bool bad;
     const uint32_t n = fwd_count(P, bad), tile = blockIdx.x, ntiles = (n + T - 1) / T;
-    if (tile >= ntiles || *(volatile const uint32_t*)(P.totals + 2) == P.epoch) return;     // nothing to place, or it does not fit
+    if (tile >= ntiles || *(volatile const uint32_t*)(P.totals + 2) == P.place.epoch) return;     // nothing to place, or it does not fit
     const uint32_t j0 = tile * T, nq = min((uint32_t)T, n - j0), j = j0 + tid;
     if (tid < (int)nq) { s_rt[tid] = P.route[j]; s_len[tid] = P.ulen[j]; }
     __syncthreads();
@@ -822,7 +819,7 @@ struct MatchParams {
     uint32_t* win;                                    // [j]: earliest accepted arrival index (NO_MATCH between calls)
     uint8_t* up; uint32_t up_cap; uint32_t* up_off;
     uint32_t* totals;                                 // {response bytes, misses answered, overflow marker, done marker}
-    unsigned long long* desc; uint32_t* counter; uint32_t ntiles_cap, epoch;
+    Place place;
 };
 
 __global__ void __launch_bounds__(256) match_kernel(const MatchParams P) {
@@ -852,7 +849,7 @@ __global__ void __launch_bounds__(T) match_gather_kernel(const MatchParams P) {
             if (len > 65535u) { len = 0; w = NO_MATCH; }
         }
         const TileScan sc = cta_scan<true>(len, w != NO_MATCH ? 1u : 0u, s_wsum, s_wsum2, lane, warp);
-        const uint64_t ex = place_tile<true>(P.desc, P.ntiles_cap, tile, sc.tot, sc.tot2, s_prefix, tid);
+        const uint64_t ex = place_tile<true>(P.place, tile, sc.tot, sc.tot2, s_prefix, tid);
         const uint64_t base = ex & ((1ull << D_MISS_SHIFT) - 1);
         const bool ovf = base + sc.tot > (uint64_t)P.up_cap;
         if (tid < (int)nq) {
@@ -860,13 +857,13 @@ __global__ void __launch_bounds__(T) match_gather_kernel(const MatchParams P) {
             P.up_off[j] = at;
             if (!ovf && len) { const uint8_t* src = P.resp + P.resp_off[w]; for (uint32_t i = 0; i < len; i++) P.up[at + i] = src[i]; }
         }
-        if (ovf && tid == 0) P.totals[2] = P.epoch;
+        if (ovf && tid == 0) P.totals[2] = P.place.epoch;
     }
     if (warp == 0)
-        self_clean<true>(P.desc, P.counter, ntiles, P.ntiles_cap, lane, [&](unsigned long long cur) {
+        self_clean<true>(P.place, ntiles, lane, [&](unsigned long long cur) {
             const uint32_t tb = (uint32_t)(cur & ((1ull << D_MISS_SHIFT) - 1));
-            P.up_off[n] = tb; P.totals[0] = tb; P.totals[1] = (uint32_t)(cur >> D_MISS_SHIFT); P.totals[3] = P.epoch;
-            if (bad) P.totals[2] = P.epoch;
+            P.up_off[n] = tb; P.totals[0] = tb; P.totals[1] = (uint32_t)(cur >> D_MISS_SHIFT); P.totals[3] = P.place.epoch;
+            if (bad) P.totals[2] = P.place.epoch;
         });
 }
 
@@ -1152,17 +1149,25 @@ struct bb_engine {
 // A launch's placement scratch: desc[max_tiles] (each tile's published prefix), the arrival cursor in desc[max_tiles], the
 // claim counter in the word after it, and two spare words.
 static size_t place_scratch_bytes(const bb_engine* e) { return ((size_t)e->max_tiles + 4) * 8; }
-// The placement fields of a kernel's parameters (Params, RelayParams, FwdParams, MatchParams), with the launch's epoch.
+// The placement block of a kernel's parameters (Params, RelayParams, LogParams, FwdParams, MatchParams), with the
+// launch's epoch.
 template <class P> static void place_params(bb_engine* e, unsigned long long* desc, P& p) {
-    p.desc = desc; p.counter = (uint32_t*)(desc + e->max_tiles + 1); p.ntiles_cap = e->max_tiles;
-    p.epoch = (uint32_t)(++e->epoch);
+    p.place = { desc, e->max_tiles, (uint32_t)(++e->epoch) };
 }
 
-// One piece of the staging block: the device pointer it sets and the bytes it needs.
+// A tile kernel's grid: one block per tile, and one for an empty call, which still reports its totals.
+static uint32_t tile_grid(uint32_t n) { return n ? (n + bbk::T - 1) / bbk::T : 1u; }
+
+// One piece of the staging block: the device pointer it sets, the bytes it needs, and the host bytes, if any, copied into
+// it before the launch (`src`) or out of it after the launch (`dst`; OUT_BYTES: as many as the launch's totals[0]).
+constexpr size_t OUT_BYTES = ~(size_t)0;
 struct Piece {
     void** at; size_t bytes;
+    const void* src = nullptr; void* dst = nullptr; size_t copy = 0;
     template <class T> Piece(T*& p, size_t n) : at((void**)&p), bytes(n) {}
 };
+template <class T> static Piece h2d(T*& p, size_t n, const void* src, size_t copy) { Piece c(p, n); c.src = src; c.copy = copy; return c; }
+template <class T> static Piece d2h(T*& p, size_t n, void* dst, size_t copy) { Piece c(p, n); c.dst = dst; c.copy = copy; return c; }
 // Cuts `pieces` out of the staging block in order, each 256-byte aligned as an allocation of its own would be; the block
 // grows (never shrinks) when they need more.  A kernel marks an overflow only by writing its epoch into totals[2], so every
 // call lists its totals first and a new block starts with them zeroed: that word never holds stale bytes of other pieces.
@@ -1178,6 +1183,32 @@ static int stage(bb_engine* e, std::initializer_list<Piece> pieces) {
     }
     size_t at = 0;
     for (const Piece& p : pieces) { *p.at = e->staging + at; at += up(p.bytes); }
+    return BB_OK;
+}
+
+// A synchronous call on the engine's sync context: stages `pieces` (the launch's totals first), copies their host sources
+// in, runs launch(), reads back tot_bytes (at most 20) of the totals, and hands them to check(), which returns BB_OK or
+// the call's error.  Then it copies the pieces' results back, and waits for them only when there were any.
+template <class Launch, class Check>
+static int run_sync(bb_engine* e, size_t tot_bytes, std::initializer_list<Piece> pieces, Launch launch, Check check) {
+    int rc = stage(e, pieces);
+    if (rc != BB_OK) return rc;
+    const cudaStream_t st = e->sync.stream;
+    for (const Piece& p : pieces)
+        if (p.src && p.copy) CK(cudaMemcpyAsync(*p.at, p.src, p.copy, cudaMemcpyHostToDevice, st));
+    rc = launch();
+    if (rc != BB_OK) return rc;
+    uint32_t tot[5];
+    CK(cudaMemcpyAsync(tot, *pieces.begin()->at, tot_bytes, cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    rc = check(tot);
+    if (rc != BB_OK) return rc;
+    bool copied = false;
+    for (const Piece& p : pieces) {
+        const size_t bytes = p.copy == OUT_BYTES ? tot[0] : p.copy;
+        if (p.dst && bytes) { CK(cudaMemcpyAsync(p.dst, *p.at, bytes, cudaMemcpyDeviceToHost, st)); copied = true; }
+    }
+    if (copied) CK(cudaStreamSynchronize(st));
     return BB_OK;
 }
 
@@ -1406,7 +1437,7 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     // An empty batch still runs one block: its last-block path writes out_off[0] = 0 and totals {0, 0, -, epoch}, so a
     // caller polling the done marker sees this launch finish like any other (no tiles, so nothing to stamp)
     if (n == 0) P.stage_log = nullptr;
-    const uint32_t grid = P.ntiles ? P.ntiles : 1u;
+    const uint32_t grid = tile_grid(n);
     // Which variant: the service variant (copy jobs + emit rounds, a tile per SM fewer) pays off when answers are long.  Decided
     // from the latest batch whose totals are known: the host path learns them in bb_resolve_wait, the device path from a
     // 16-byte copy of d_totals that follows every launch (looked at only once its epoch has landed: no synchronisation).
@@ -1421,7 +1452,7 @@ static int launch(bb_engine* e, unsigned long long* desc, const uint8_t* d_pkts,
     // profile 0: the service variant when the latest known batch averaged >= 96 response bytes per query (its tiles are then
     // "big": more than one staging window, where copy jobs pay off; config 2's 64-byte answers stay on the small variant)
     const bool svc = e->profile == 2 || (e->profile == 0 && e->mean_resp >= 96);
-    P.fb = (feedback && e->profile == 0) ? e->h_fb + 4 * (P.epoch % bb_engine::FB) : nullptr;
+    P.fb = (feedback && e->profile == 0) ? e->h_fb + 4 * (P.place.epoch % bb_engine::FB) : nullptr;
     // no memsets: the kernel leaves desc/counter zeroed for the next launch (self-cleaning)
     resolve_launch(P, grid, st, e->ordered, svc);
     CK(cudaGetLastError());
@@ -1469,9 +1500,8 @@ static int relay_launch(bb_engine* e, const StreamCtx& c, const uint8_t* d_q, co
     P.q = d_q; P.q_off = d_q_off; P.up = d_up; P.up_off = d_up_off; P.n = n;
     P.out = out; P.out_cap = out_cap; P.out_off = out_off; P.out_len = out_len; P.status = status; P.totals = totals; P.bounce = bounce;
     place_params(e, c.desc, P); P.tcp = (flags & BB_BATCH_TCP) ? 1u : 0u;
-    const uint32_t ntiles = (n + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;   // an empty batch still reports its totals
-    if (e->ordered) bbk::relay_kernel<true><<<grid, bbk::T, 0, c.stream>>>(P);
-    else bbk::relay_kernel<false><<<grid, bbk::T, 0, c.stream>>>(P);
+    const auto kernel = e->ordered ? bbk::relay_kernel<true> : bbk::relay_kernel<false>;
+    kernel<<<tile_grid(n), bbk::T, 0, c.stream>>>(P);
     CK(cudaGetLastError());
     e->launches++;
     return BB_OK;
@@ -1499,31 +1529,19 @@ int bb_relay_batch(bb_engine* e, const uint8_t* q_pkts, const uint32_t* q_off, c
     // device output is then the kernel's bounce buffer, and the offsets, lengths and statuses need no device copy
     const void* outs[4] = { out, out_off, out_len, status };
     const bool zc = e->r_pinned.check(outs, 4) && n != 0;
+    auto res = [zc](auto*& d, size_t bytes, void* h, size_t copy) { return zc ? Piece(d, 0) : d2h(d, bytes, h, copy); };
+    const size_t nb = n;
     uint8_t *d_q, *d_up, *d_out, *d_status; uint32_t *d_totals, *d_qoff, *d_upoff, *d_out_off; uint16_t* d_out_len;
-    int rc = stage(e, { { d_totals, 16 }, { d_q, (size_t)qbytes + 64 }, { d_qoff, ((size_t)n + 1) * 4 }, { d_up, (size_t)ubytes + 64 },
-                        { d_upoff, ((size_t)n + 1) * 4 }, { d_out, (size_t)ocap + 64 }, { d_out_off, zc ? 0 : ((size_t)n + 1) * 4 },
-                        { d_out_len, zc ? 0 : (size_t)n * 2 + 16 }, { d_status, zc ? 0 : (size_t)n + 16 } });
-    if (rc != BB_OK) return rc;
-    const StreamCtx& c = e->sync;
-    if (qbytes) CK(cudaMemcpyAsync(d_q, q_pkts, qbytes, cudaMemcpyHostToDevice, c.stream));
-    if (ubytes) CK(cudaMemcpyAsync(d_up, up_pkts, ubytes, cudaMemcpyHostToDevice, c.stream));
-    CK(cudaMemcpyAsync(d_qoff, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
-    CK(cudaMemcpyAsync(d_upoff, up_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
-    rc = relay_launch(e, c, d_q, d_qoff, d_up, d_upoff, n, flags, zc ? out : d_out, (uint32_t)ocap, zc ? out_off : d_out_off,
-                      zc ? out_len : d_out_len, zc ? status : d_status, d_totals, zc ? d_out : nullptr);
-    if (rc != BB_OK) return rc;
-    const uint32_t epoch = (uint32_t)e->epoch;
-    uint32_t tot[4];
-    CK(cudaMemcpyAsync(tot, d_totals, 16, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    if (tot[2] == epoch || tot[0] > out_cap) return BB_ERR_CAPACITY;
-    if (zc) return BB_OK;                        // everything is already in the caller's buffers
-    if (tot[0]) CK(cudaMemcpyAsync(out, d_out, tot[0], cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaMemcpyAsync(out_off, d_out_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
-    if (n) CK(cudaMemcpyAsync(out_len, d_out_len, (size_t)n * 2, cudaMemcpyDeviceToHost, c.stream));
-    if (n) CK(cudaMemcpyAsync(status, d_status, n, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    return BB_OK;
+    return run_sync(e, 16,
+        { { d_totals, 16 },
+          h2d(d_q, (size_t)qbytes + 64, q_pkts, qbytes), h2d(d_qoff, (nb + 1) * 4, q_off, (nb + 1) * 4),
+          h2d(d_up, (size_t)ubytes + 64, up_pkts, ubytes), h2d(d_upoff, (nb + 1) * 4, up_off, (nb + 1) * 4),
+          d2h(d_out, (size_t)ocap + 64, zc ? nullptr : out, OUT_BYTES), res(d_out_off, (nb + 1) * 4, out_off, (nb + 1) * 4),
+          res(d_out_len, nb * 2 + 16, out_len, nb * 2), res(d_status, nb + 16, status, nb) },
+        [&] { return relay_launch(e, e->sync, d_q, d_qoff, d_up, d_upoff, n, flags, zc ? out : d_out, (uint32_t)ocap,
+                                  zc ? out_off : d_out_off, zc ? out_len : d_out_len, zc ? status : d_status, d_totals,
+                                  zc ? d_out : nullptr); },
+        [&](const uint32_t* tot) { return tot[2] == (uint32_t)e->epoch || tot[0] > out_cap ? BB_ERR_CAPACITY : BB_OK; });
 }
 
 int bb_relay_batch_device(bb_engine* e, const uint8_t* d_q_pkts, const uint32_t* d_q_off, const uint8_t* d_up_pkts,
@@ -1549,9 +1567,8 @@ static int log_launch(bb_engine* e, const StreamCtx& c, const uint8_t* resp, uin
     P.log = log; P.log_cap = log_cap; P.log_off = log_off; P.log_len = log_len; P.head_len = head_len; P.summary = summary;
     P.totals = totals; P.bounce = bounce;
     place_params(e, c.desc, P);
-    const uint32_t ntiles = (n + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;   // an empty set still reports its totals
-    if (e->ordered) bbk::log_kernel<true><<<grid, bbk::T, 0, c.stream>>>(P);
-    else bbk::log_kernel<false><<<grid, bbk::T, 0, c.stream>>>(P);
+    const auto kernel = e->ordered ? bbk::log_kernel<true> : bbk::log_kernel<false>;
+    kernel<<<tile_grid(n), bbk::T, 0, c.stream>>>(P);
     CK(cudaGetLastError());
     e->launches++;
     return BB_OK;
@@ -1564,39 +1581,24 @@ int bb_log_batch(bb_engine* e, const uint8_t* resp, uint32_t resp_bytes, const u
     if (n && (!out_off || !out_len || !status || !log || !log_len || !head_len || (resp_bytes && !resp))) return BB_ERR_ARG;
     CK(cudaSetDevice(e->device));
     // zero-copy results when every output buffer is pinned host memory, as bb_relay_batch: the device log is then the
-    // kernel's bounce buffer.  Without a summary the log buffer stands in for it, so that the check always covers five.
+    // kernel's bounce buffer, and the other arrays need no device copy.  Without a summary the log buffer stands in for it,
+    // so that the check always covers five.
     const void* outs[5] = { log, log_off, log_len, head_len, summary ? (const void*)summary : log };
     const bool zc = e->l_pinned.check(outs, 5) && n != 0;
+    auto res = [zc](auto*& d, size_t bytes, void* h, size_t copy) { return zc ? Piece(d, 0) : d2h(d, bytes, h, copy); };
+    const size_t nb = n;
     uint8_t *d_resp, *d_status, *d_log; uint32_t *d_totals, *d_off, *d_log_off, *d_log_len, *d_summary; uint16_t *d_len, *d_head_len;
-    int rc = stage(e, { { d_totals, 16 }, { d_resp, (size_t)resp_bytes + 64 }, { d_off, (size_t)n * 4 + 16 }, { d_len, (size_t)n * 2 + 16 },
-                        { d_status, (size_t)n + 16 }, { d_log, (size_t)log_cap + 64 }, { d_log_off, zc ? 0 : ((size_t)n + 1) * 4 },
-                        { d_log_len, zc ? 0 : (size_t)n * 4 + 16 }, { d_head_len, zc ? 0 : (size_t)n * 2 + 16 },
-                        { d_summary, zc || !summary ? 0 : (size_t)n * 4 + 16 } });
-    if (rc != BB_OK) return rc;
-    const StreamCtx& c = e->sync;
-    if (resp_bytes) CK(cudaMemcpyAsync(d_resp, resp, resp_bytes, cudaMemcpyHostToDevice, c.stream));
-    if (n) {
-        CK(cudaMemcpyAsync(d_off, out_off, (size_t)n * 4, cudaMemcpyHostToDevice, c.stream));
-        CK(cudaMemcpyAsync(d_len, out_len, (size_t)n * 2, cudaMemcpyHostToDevice, c.stream));
-        CK(cudaMemcpyAsync(d_status, status, n, cudaMemcpyHostToDevice, c.stream));
-    }
-    rc = log_launch(e, c, d_resp, resp_bytes, nullptr, d_off, d_len, d_status, n, zc ? log : d_log, log_cap, zc ? log_off : d_log_off,
-                    zc ? log_len : d_log_len, zc ? head_len : d_head_len, zc ? summary : summary ? d_summary : nullptr, d_totals,
-                    zc ? d_log : nullptr);
-    if (rc != BB_OK) return rc;
-    const uint32_t epoch = (uint32_t)e->epoch;
-    uint32_t tot[4];
-    CK(cudaMemcpyAsync(tot, d_totals, 16, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    if (tot[2] == epoch || tot[0] > log_cap) return BB_ERR_CAPACITY;
-    if (zc) return BB_OK;                        // everything is already in the caller's buffers
-    if (tot[0]) CK(cudaMemcpyAsync(log, d_log, tot[0], cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaMemcpyAsync(log_off, d_log_off, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
-    if (n) CK(cudaMemcpyAsync(log_len, d_log_len, (size_t)n * 4, cudaMemcpyDeviceToHost, c.stream));
-    if (n) CK(cudaMemcpyAsync(head_len, d_head_len, (size_t)n * 2, cudaMemcpyDeviceToHost, c.stream));
-    if (n && summary) CK(cudaMemcpyAsync(summary, d_summary, (size_t)n * 4, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    return BB_OK;
+    return run_sync(e, 16,
+        { { d_totals, 16 },
+          h2d(d_resp, (size_t)resp_bytes + 64, resp, resp_bytes), h2d(d_off, nb * 4 + 16, out_off, nb * 4),
+          h2d(d_len, nb * 2 + 16, out_len, nb * 2), h2d(d_status, nb + 16, status, nb),
+          d2h(d_log, (size_t)log_cap + 64, zc ? nullptr : log, OUT_BYTES), res(d_log_off, (nb + 1) * 4, log_off, (nb + 1) * 4),
+          res(d_log_len, nb * 4 + 16, log_len, nb * 4), res(d_head_len, nb * 2 + 16, head_len, nb * 2),
+          res(d_summary, summary ? nb * 4 + 16 : 0, summary, nb * 4) },
+        [&] { return log_launch(e, e->sync, d_resp, resp_bytes, nullptr, d_off, d_len, d_status, n, zc ? log : d_log, log_cap,
+                                zc ? log_off : d_log_off, zc ? log_len : d_log_len, zc ? head_len : d_head_len,
+                                zc ? summary : summary ? d_summary : nullptr, d_totals, zc ? d_log : nullptr); },
+        [&](const uint32_t* tot) { return tot[2] == (uint32_t)e->epoch || tot[0] > log_cap ? BB_ERR_CAPACITY : BB_OK; });
 }
 
 int bb_log_batch_device(bb_engine* e, const uint8_t* d_resp, uint32_t resp_bytes, const uint32_t* d_resp_totals,
@@ -1640,7 +1642,7 @@ static int forward_launch(bb_engine* e, StreamCtx& c, const uint8_t* pkts, const
     P.uq = uq; P.uq_cap = uq_cap; P.uq_off = uq_off; P.order = order; P.group_off = group_off; P.route = route;
     P.q = q; P.q_cap = q_cap; P.q_off = q_off; P.totals = totals; P.hist = c.hist; P.ulen = c.ulen;
     place_params(e, c.desc, P);
-    const uint32_t ntiles = (n_cap + bbk::T - 1) / bbk::T, grid = ntiles ? ntiles : 1u;     // an empty call still reports its totals
+    const uint32_t grid = tile_grid(n_cap);
     bbk::forward_kernel<<<grid, bbk::T, 0, c.stream>>>(P);
     bbk::forward_group_kernel<<<1, bbk::FG_T, 0, c.stream>>>(P);
     bbk::forward_scatter_kernel<<<grid, bbk::T, 0, c.stream>>>(P);
@@ -1662,8 +1664,7 @@ static int match_launch(bb_engine* e, StreamCtx& c, const uint8_t* resp, const u
     P.up = up; P.up_cap = up_cap; P.up_off = up_off; P.totals = totals;
     place_params(e, c.desc, P);
     if (n_resp) bbk::match_kernel<<<(n_resp + 255) / 256, 256, 0, c.stream>>>(P);
-    const uint32_t ntiles = (n_cap + bbk::T - 1) / bbk::T;
-    bbk::match_gather_kernel<<<ntiles ? ntiles : 1u, bbk::T, 0, c.stream>>>(P);
+    bbk::match_gather_kernel<<<tile_grid(n_cap), bbk::T, 0, c.stream>>>(P);
     CK(cudaGetLastError());
     e->launches += n_resp ? 2 : 1;
     return BB_OK;
@@ -1675,31 +1676,21 @@ int bb_forward_batch(bb_engine* e, const uint8_t* pkts, const uint32_t* pkt_off,
     if (n && (!order || !route || !uq || (pkt_off[n] && !pkts) || !offsets_ok(pkt_off, n))) return BB_ERR_ARG;
     const uint32_t bytes = pkt_off[n];
     CK(cudaSetDevice(e->device));
+    const size_t nb = n;
     uint8_t *d_pk, *d_uq, *d_route, *d_q; uint32_t *d_tot, *d_pkoff, *d_uqoff, *d_order, *d_goff, *d_qoff;
-    int rc = stage(e, { { d_tot, 32 }, { d_pk, (size_t)bytes + 64 }, { d_pkoff, ((size_t)n + 1) * 4 }, { d_uq, (size_t)bytes + 64 },
-                        { d_uqoff, ((size_t)n + 1) * 4 }, { d_order, (size_t)n * 4 + 16 }, { d_goff, (bbk::NROUTE + 1) * 4 },
-                        { d_route, (size_t)n + 16 }, { d_q, (size_t)bytes + 64 }, { d_qoff, ((size_t)n + 1) * 4 } });
-    if (rc != BB_OK) return rc;
-    StreamCtx& c = e->sync;
-    if (bytes) CK(cudaMemcpyAsync(d_pk, pkts, bytes, cudaMemcpyHostToDevice, c.stream));
-    CK(cudaMemcpyAsync(d_pkoff, pkt_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
     // an upstream query is never longer than its client query: the device buffers hold the whole batch
-    rc = forward_launch(e, c, d_pk, d_pkoff, nullptr, nullptr, n, n, id_key, d_uq, bytes, d_uqoff, d_order, d_goff, d_route, d_q, bytes,
-                        d_qoff, d_tot);
-    if (rc != BB_OK) return rc;
-    const uint32_t epoch = (uint32_t)e->epoch;
-    uint32_t tot[5];
-    CK(cudaMemcpyAsync(tot, d_tot, 20, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    if (tot[2] == epoch) { g_cuda_err = "forward: device buffers overflowed"; return BB_ERR_CUDA; }
-    if (tot[0] > uq_cap) return BB_ERR_CAPACITY;
-    if (tot[0]) CK(cudaMemcpyAsync(uq, d_uq, tot[0], cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaMemcpyAsync(uq_off, d_uqoff, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaMemcpyAsync(group_off, d_goff, (bbk::NROUTE + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
-    if (n) CK(cudaMemcpyAsync(order, d_order, (size_t)n * 4, cudaMemcpyDeviceToHost, c.stream));
-    if (n) CK(cudaMemcpyAsync(route, d_route, n, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    return BB_OK;
+    return run_sync(e, 20,
+        { { d_tot, 32 },
+          h2d(d_pk, (size_t)bytes + 64, pkts, bytes), h2d(d_pkoff, (nb + 1) * 4, pkt_off, (nb + 1) * 4),
+          d2h(d_uq, (size_t)bytes + 64, uq, OUT_BYTES), d2h(d_uqoff, (nb + 1) * 4, uq_off, (nb + 1) * 4),
+          d2h(d_order, nb * 4 + 16, order, nb * 4), d2h(d_goff, (bbk::NROUTE + 1) * 4, group_off, (bbk::NROUTE + 1) * 4),
+          d2h(d_route, nb + 16, route, nb), { d_q, (size_t)bytes + 64 }, { d_qoff, (nb + 1) * 4 } },
+        [&] { return forward_launch(e, e->sync, d_pk, d_pkoff, nullptr, nullptr, n, n, id_key, d_uq, bytes, d_uqoff, d_order, d_goff,
+                                    d_route, d_q, bytes, d_qoff, d_tot); },
+        [&](const uint32_t* tot) {
+            if (tot[2] == (uint32_t)e->epoch) { g_cuda_err = "forward: device buffers overflowed"; return BB_ERR_CUDA; }
+            return tot[0] > uq_cap ? BB_ERR_CAPACITY : BB_OK;
+        });
 }
 
 int bb_forward_batch_device(bb_engine* e, const uint8_t* d_pkts, const uint32_t* d_pkt_off, const uint32_t* d_miss_idx,
@@ -1725,32 +1716,18 @@ int bb_match_upstreams(bb_engine* e, const uint8_t* resp, const uint32_t* resp_o
     if (n && (!route || (q_off[n] && !q_pkts) || !offsets_ok(q_off, n))) return BB_ERR_ARG;
     const uint32_t rbytes = resp_off[n_resp], qbytes = q_off[n];
     CK(cudaSetDevice(e->device));
+    const size_t nb = n, nr = n_resp;
     uint8_t *d_resp, *d_q, *d_route, *d_up; uint32_t *d_tot, *d_respoff, *d_ip, *d_qoff, *d_upoff; uint16_t* d_port;
-    int rc = stage(e, { { d_tot, 32 }, { d_resp, (size_t)rbytes + 64 }, { d_respoff, ((size_t)n_resp + 1) * 4 },
-                        { d_ip, (size_t)n_resp * 4 + 16 }, { d_port, (size_t)n_resp * 2 + 16 }, { d_q, (size_t)qbytes + 64 },
-                        { d_qoff, ((size_t)n + 1) * 4 }, { d_route, (size_t)n + 16 }, { d_up, (size_t)rbytes + 64 },
-                        { d_upoff, ((size_t)n + 1) * 4 } });
-    if (rc != BB_OK) return rc;
-    StreamCtx& c = e->sync;
-    if (rbytes) CK(cudaMemcpyAsync(d_resp, resp, rbytes, cudaMemcpyHostToDevice, c.stream));
-    CK(cudaMemcpyAsync(d_respoff, resp_off, ((size_t)n_resp + 1) * 4, cudaMemcpyHostToDevice, c.stream));
-    if (n_resp) CK(cudaMemcpyAsync(d_ip, src_ip, (size_t)n_resp * 4, cudaMemcpyHostToDevice, c.stream));
-    if (n_resp) CK(cudaMemcpyAsync(d_port, src_port, (size_t)n_resp * 2, cudaMemcpyHostToDevice, c.stream));
-    if (qbytes) CK(cudaMemcpyAsync(d_q, q_pkts, qbytes, cudaMemcpyHostToDevice, c.stream));
-    CK(cudaMemcpyAsync(d_qoff, q_off, ((size_t)n + 1) * 4, cudaMemcpyHostToDevice, c.stream));
-    if (n) CK(cudaMemcpyAsync(d_route, route, n, cudaMemcpyHostToDevice, c.stream));
     // the winners are distinct responses: their bytes fit a buffer of all the responses
-    rc = match_launch(e, c, d_resp, d_respoff, d_ip, d_port, n_resp, d_q, d_qoff, d_route, nullptr, n, n, id_key, d_up, rbytes, d_upoff,
-                      d_tot);
-    if (rc != BB_OK) return rc;
-    uint32_t tot[4];
-    CK(cudaMemcpyAsync(tot, d_tot, 16, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    if (tot[0] > up_cap) return BB_ERR_CAPACITY;
-    if (tot[0]) CK(cudaMemcpyAsync(up, d_up, tot[0], cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaMemcpyAsync(up_off, d_upoff, ((size_t)n + 1) * 4, cudaMemcpyDeviceToHost, c.stream));
-    CK(cudaStreamSynchronize(c.stream));
-    return BB_OK;
+    return run_sync(e, 16,
+        { { d_tot, 32 },
+          h2d(d_resp, (size_t)rbytes + 64, resp, rbytes), h2d(d_respoff, (nr + 1) * 4, resp_off, (nr + 1) * 4),
+          h2d(d_ip, nr * 4 + 16, src_ip, nr * 4), h2d(d_port, nr * 2 + 16, src_port, nr * 2),
+          h2d(d_q, (size_t)qbytes + 64, q_pkts, qbytes), h2d(d_qoff, (nb + 1) * 4, q_off, (nb + 1) * 4),
+          h2d(d_route, nb + 16, route, nb), d2h(d_up, (size_t)rbytes + 64, up, OUT_BYTES), d2h(d_upoff, (nb + 1) * 4, up_off, (nb + 1) * 4) },
+        [&] { return match_launch(e, e->sync, d_resp, d_respoff, d_ip, d_port, n_resp, d_q, d_qoff, d_route, nullptr, n, n, id_key, d_up,
+                                  rbytes, d_upoff, d_tot); },
+        [&](const uint32_t* tot) { return tot[0] > up_cap ? BB_ERR_CAPACITY : BB_OK; });
 }
 
 int bb_match_upstreams_device(bb_engine* e, const uint8_t* d_resp, const uint32_t* d_resp_off, const uint32_t* d_src_ip,
@@ -1995,8 +1972,7 @@ int bb_shard_route_push_ex(bb_shard* s, const uint8_t* d_pkts, const uint32_t* d
     // stream order before the launch, and the last block publishes it in every header of the step.
     if (flags & BB_BATCH_TCP) CK(cudaMemsetAsync(s->err, bbk::HDR_TCP, 1, (cudaStream_t)stream));
     // n == 0 still publishes empty region headers (one block, no queries)
-    const uint32_t grid = n ? (n + bbk::T - 1) / bbk::T : 1;
-    bbk::route_push_kernel<<<grid, bbk::T, 0, (cudaStream_t)stream>>>(A);
+    bbk::route_push_kernel<<<tile_grid(n), bbk::T, 0, (cudaStream_t)stream>>>(A);
     CK(cudaGetLastError());
     e->launches++;
     return BB_OK;
@@ -2037,7 +2013,7 @@ int bb_shard_resolve(bb_shard* s, uint64_t seed, int wait_for_peers, void* strea
     P.status_stride = s->status_stride; P.miss_stride = s->miss_stride; P.totals_stride = s->totals_stride; P.desc_stride = s->desc_stride;
     resolve_launch(P, dim3(P.ntiles, s->nranks), main, e->ordered, false);
     CK(cudaGetLastError());
-    s->resolve_epoch = P.epoch;
+    s->resolve_epoch = P.place.epoch;
     e->launches++;
     return BB_OK;
 }

@@ -33,14 +33,21 @@ enum { RC_NOERROR = 0, RC_SERVFAIL = 2, RC_NXDOMAIN = 3, RC_NOTIMP = 4, RC_REFUS
 enum { QT_A = 1, QT_SOA = 6, QT_PTR = 12, QT_SRV = 33, QT_OPT = 41 };
 enum { RK_NONE = 0, RK_HEADER = 1, RK_A1 = 2, RK_PTR = 3, RK_SOA = 4, RK_SVC_A = 5, RK_SVC_SRV = 6 };
 
+// A tile kernel's placement state: desc[0, ntiles_cap) holds each tile's published prefix, desc[ntiles_cap] the arrival
+// cursor, and the upper word of desc[ntiles_cap + 1] the finished-block counter; epoch is the launch number, which marks
+// totals[2] (overflow) / totals[3] (done) of THIS launch.
+struct Place {
+    unsigned long long* desc;
+    uint32_t ntiles_cap, epoch;
+};
+
 struct Params {
     const uint8_t* pkts; const uint32_t* pkt_off; uint32_t n;
     uint64_t seed; uint32_t qidx_base;
     uint8_t* out; uint32_t out_cap; uint32_t* out_off; uint16_t* out_len; uint8_t* status; uint32_t* miss_idx; uint32_t* totals;
     const Slot* table; uint32_t mask; const uint8_t* arena; int ready;
     const EngineConst* eng;
-    unsigned long long* desc; uint32_t* counter; uint32_t ntiles, ntiles_cap;   // desc[ntiles_cap] = arrival cursor
-    uint32_t epoch;          // launch number: marks totals[2] (overflow) / totals[3] (done) of THIS launch
+    Place place; uint32_t ntiles;
     unsigned long long* stage_log;   // optional [ntiles][8] globaltimer stamps (bb_engine_set_stage_log)
     const uint32_t* n_dev;           // when set, the batch size is read from device memory (routed batches)
     const uint32_t* qidx_map;        // when set, query i's shuffle index is qidx_map[i] (routed batches)

@@ -1,7 +1,8 @@
 """The synchronous host-buffer calls of one recursion engine share one device staging block (DESIGN.md section 13):
-resolve_batch, relay_batch (pageable and pinned results), forward_batch and match_upstreams, interleaved, bit-exact
-against the CPU oracles.  Batch sizes go small, large, small, large, so each call cuts its pieces out of a block that an
-earlier call of another kind grew and left full of its own bytes.  Device-form relay and forward calls on two other
+resolve_batch, relay_batch (pageable and pinned results), forward_batch, match_upstreams and log_batch (pageable, and
+pinned with and without a summary), interleaved, bit-exact against the CPU oracles and the query log restatement.
+Batch sizes go small, large, small, large, so each call cuts its pieces out of a block that an earlier call of another
+kind grew and left full of its own bytes.  Device-form relay and forward calls on two other
 streams run alongside, on their own placement and forward scratch.  A relay that overflows its capacity is followed by an
 exact one on the same engine."""
 import random
@@ -11,6 +12,7 @@ import pytest
 
 import forward_oracle as O
 import forwardgen as G
+import query_log_ref as L
 import relay_oracle
 import relaygen as RG
 from binder_b200 import synth
@@ -19,6 +21,7 @@ from binder_b200.engine import Engine
 from oracle_lib import Oracle
 from test_gpu_forward import _zone, chain_batch, same
 from test_gpu_parity import compare
+from test_gpu_query_log import records
 from test_gpu_relay import check, pinned
 from test_relay import corpus
 
@@ -114,6 +117,29 @@ def relay_pinned(e, mq, moff, up, up_off, want):
             lib().bb_host_free(p)
 
 
+def log_pageable(e, rs):
+    """The query log of result set rs, with summaries, against the restatement."""
+    assert records(e.log_batch(*rs, summary=True)) == L.log_set(*rs, 'foo.com')
+
+
+def log_pinned(e, rs):
+    """The query log of result set rs into pinned buffers, without and with a summary, against the restatement."""
+    want = L.log_set(*rs, 'foo.com')
+    n, total = len(rs[3]), sum(len(h) + len(b) for h, b, _ in want)
+    for summary in (False, True):
+        bufs = [pinned(total + 64, np.uint8), pinned(n + 1, np.uint32), pinned(n, np.uint32), pinned(n, np.uint16),
+                pinned(n, np.uint32)]
+        try:
+            arrs = [b for b, _ in bufs]
+            if not summary:
+                arrs[4] = None
+            res = e.log_batch(*rs, summary=summary, buffers=tuple(arrs))
+            assert records(res if summary else res + (np.array([w[2] for w in want], np.uint32),)) == want
+        finally:
+            for _, p in bufs:
+                lib().bb_host_free(p)
+
+
 def test_gpu_host_staging_shared_across_calls():
     orc = Oracle('foo.com', 'dc1', True, snapshot=_zone('dc1', 200))
     orc.set_recursion_filter(REGION, DCS, True)
@@ -125,7 +151,9 @@ def test_gpu_host_staging_shared_across_calls():
     for r, n in enumerate((300, 60000, 40, 45000)):
         dev.enqueue()
         data, off, want, mq, moff = misses(orc, n, 10 + r)
-        compare(e.resolve_batch(data, off, seed=10 + r), want, data, off, True)
+        res = e.resolve_batch(data, off, seed=10 + r)
+        compare(res, want, data, off, True)
+        log_pageable(e, res[:4])
         key = 0xC0FFEE12345 * (r + 1)
         fwd = O.forward_batch(tb, mq, moff, key)
         same(e.forward_batch(mq, moff, key), fwd)
@@ -133,8 +161,10 @@ def test_gpu_host_staging_shared_across_calls():
         up, up_off = O.match_upstreams(tb, *args)
         same(e.match_upstreams(*args), (up, up_off))
         relayed = relay_oracle.relay_batch(mq, moff, up, up_off, nthreads=8)
-        check(e.relay_batch(mq, moff, up, up_off), relayed, True)
+        rel = e.relay_batch(mq, moff, up, up_off)
+        check(rel, relayed, True)
         relay_pinned(e, mq, moff, up, up_off, relayed)
+        log_pinned(e, rel)
         dev.check()
     # one byte short of the replies: BB_ERR_CAPACITY, then the exact capacity on the same engine
     m = len(moff) - 1
