@@ -307,7 +307,11 @@ static napi_value MatchUpstreams(napi_env env, napi_callback_info info) {
 //   tcpHubEof(hub, session)          tcpHubFlush(hub, seed: BigInt) -> misses {pkts: Buffer, pktOff: Uint32Array, session: Uint32Array}
 //   tcpHubOutput(hub, session) -> {out: Buffer, closable: Uint8Array(1)}     tcpHubConsume(hub, session, nBytes)
 //   tcpHubClose(hub, session)        tcpHubRelay(hub, pkts, pktOff, upstream, upOff, sessions: Uint32Array)
-//   tcpHubStats(hub) -> BigUint64Array(11)   (bb_tcp_hub_stat 0..10)
+//   tcpHubStats(hub) -> BigUint64Array(13)   (bb_tcp_hub_stat 0..12)
+//   tcpHubSetQueryLog(hub, on: bool)   tcpHubQueryLog(hub, which: 0 last flush | 1 last relay) -> the "DNS query" log records
+//       of the answers appended: {log: Buffer, logOff, logLen: Uint32Array, headLen, reqId: Uint16Array, clientIp,
+//       clientPort, session: Uint32Array, lost: Uint32Array(1)}   (bb_query_log_tcp_hub; record i = log[logOff[i] ..
+//       logOff[i] + logLen[i]), its first headLen[i] bytes the head fragment)
 static napi_value U32Array(napi_env env, const uint32_t* src, size_t n) {
     void* p; napi_value ab, t;
     if (napi_create_arraybuffer(env, n * 4, &p, &ab) != napi_ok || napi_create_typedarray(env, napi_uint32_array, n, ab, 0, &t) != napi_ok) return nullptr;
@@ -319,6 +323,29 @@ static napi_value CopyBuffer(napi_env env, const uint8_t* src, size_t n) {
     if (napi_create_buffer(env, n, &p, &b) != napi_ok) return nullptr;
     if (n) memcpy(p, src, n);
     return b;
+}
+static napi_value U16Array(napi_env env, const uint16_t* src, size_t n) {
+    void* p; napi_value ab, t;
+    if (napi_create_arraybuffer(env, n * 2, &p, &ab) != napi_ok || napi_create_typedarray(env, napi_uint16_array, n, ab, 0, &t) != napi_ok) return nullptr;
+    if (n) memcpy(p, src, n * 2);
+    return t;
+}
+// bb_query_log_records -> the object of backendQueryLog / tcpHubQueryLog (copies: the session's arrays change with its next call)
+static napi_value QueryLogObject(napi_env env, const bb_query_log_records& r) {
+    size_t end = 0;
+    for (uint32_t i = 0; i < r.n; i++) end = std::max(end, (size_t)r.log_off[i] + r.log_len[i]);
+    napi_value res;
+    if (napi_create_object(env, &res) != napi_ok) return nullptr;
+    napi_set_named_property(env, res, "log", CopyBuffer(env, r.log, end));
+    napi_set_named_property(env, res, "logOff", U32Array(env, r.log_off, r.n));
+    napi_set_named_property(env, res, "logLen", U32Array(env, r.log_len, r.n));
+    napi_set_named_property(env, res, "headLen", U16Array(env, r.head_len, r.n));
+    napi_set_named_property(env, res, "reqId", U16Array(env, r.req_id, r.n));
+    napi_set_named_property(env, res, "clientIp", U32Array(env, r.client_ip, r.n));
+    napi_set_named_property(env, res, "clientPort", U32Array(env, r.client_port, r.n));
+    if (r.session) napi_set_named_property(env, res, "session", U32Array(env, r.session, r.n));
+    napi_set_named_property(env, res, "lost", U32Array(env, &r.lost, 1));
+    return res;
 }
 static napi_value TcpHubCreate(napi_env env, napi_callback_info info) {
     size_t argc = 2; napi_value argv[2];
@@ -428,9 +455,26 @@ static napi_value TcpHubStats(napi_env env, napi_callback_info info) {
     NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
     void* h; NAPI_OK(napi_get_value_external(env, argv[0], &h));
     void* p; napi_value ab, t;
-    NAPI_OK(napi_create_arraybuffer(env, 11 * 8, &p, &ab)); NAPI_OK(napi_create_typedarray(env, napi_biguint64_array, 11, ab, 0, &t));
-    for (int i = 0; i < 11; i++) ((uint64_t*)p)[i] = bb_tcp_hub_stat((const bb_tcp_hub*)h, i);
+    NAPI_OK(napi_create_arraybuffer(env, 13 * 8, &p, &ab)); NAPI_OK(napi_create_typedarray(env, napi_biguint64_array, 13, ab, 0, &t));
+    for (int i = 0; i < 13; i++) ((uint64_t*)p)[i] = bb_tcp_hub_stat((const bb_tcp_hub*)h, i);
     return t;
+}
+static napi_value TcpHubSetQueryLog(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; NAPI_OK(napi_get_value_external(env, argv[0], &h));
+    bool on = false; NAPI_OK(napi_get_value_bool(env, argv[1], &on));
+    const int rc = bb_query_log_tcp_hub_enable((bb_tcp_hub*)h, on ? 1 : 0);
+    return rc == BB_OK ? nullptr : Throw(env, rc);
+}
+static napi_value TcpHubQueryLog(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    void* h; NAPI_OK(napi_get_value_external(env, argv[0], &h));
+    uint32_t which = 0; NAPI_OK(napi_get_value_uint32(env, argv[1], &which));
+    bb_query_log_records r;
+    const int rc = bb_query_log_tcp_hub((const bb_tcp_hub*)h, (int)std::min(which, 2u), &r);
+    return rc == BB_OK ? QueryLogObject(env, r) : Throw(env, rc);
 }
 
 // A native balancer UDP session (bb_backend_*, include/binder_b200.h):
@@ -439,7 +483,10 @@ static napi_value TcpHubStats(napi_env env, napi_callback_info info) {
 //       srcIp: Uint32Array, srcPort: Uint32Array}   (the misses, for the host's recursion; a failed batch is counted, not thrown)
 //   backendRelay(session, pkts, pktOff, upstream, upOff, dstIp: Uint32Array, dstPort: Uint32Array) -> Buffer (OUTBOUND_UDP
 //       frames of the misses' replies; a failed batch is counted, not thrown)
-//   backendStats(session) -> BigUint64Array(8)   (bb_backend_stat 0..7)
+//   backendStats(session) -> BigUint64Array(10)   (bb_backend_stat 0..9)
+//   backendSetQueryLog(session, on: bool)   backendQueryLog(session, which: 0 last feed | 1 last relay) -> the "DNS query"
+//       log records of the frames sent, one per OUTBOUND_UDP frame in order: {log: Buffer, logOff, logLen: Uint32Array,
+//       headLen, reqId: Uint16Array, clientIp, clientPort: Uint32Array, lost: Uint32Array(1)}   (bb_query_log_backend)
 //   backendDestroy(session)   (also done when the session is garbage-collected)
 struct BackendRef { bb_backend* b; };
 static bb_backend* BackendOf(napi_env env, napi_value v) {
@@ -503,9 +550,26 @@ static napi_value BackendStats(napi_env env, napi_callback_info info) {
     NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
     bb_backend* b = BackendOf(env, argv[0]); if (!b) return Throw(env, BB_ERR_ARG);
     void* p; napi_value ab, t;
-    NAPI_OK(napi_create_arraybuffer(env, 8 * 8, &p, &ab)); NAPI_OK(napi_create_typedarray(env, napi_biguint64_array, 8, ab, 0, &t));
-    for (int i = 0; i < 8; i++) ((uint64_t*)p)[i] = bb_backend_stat(b, i);
+    NAPI_OK(napi_create_arraybuffer(env, 10 * 8, &p, &ab)); NAPI_OK(napi_create_typedarray(env, napi_biguint64_array, 10, ab, 0, &t));
+    for (int i = 0; i < 10; i++) ((uint64_t*)p)[i] = bb_backend_stat(b, i);
     return t;
+}
+static napi_value BackendSetQueryLog(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    bb_backend* b = BackendOf(env, argv[0]); if (!b) return Throw(env, BB_ERR_ARG);
+    bool on = false; NAPI_OK(napi_get_value_bool(env, argv[1], &on));
+    const int rc = bb_query_log_backend_enable(b, on ? 1 : 0);
+    return rc == BB_OK ? nullptr : Throw(env, rc);
+}
+static napi_value BackendQueryLog(napi_env env, napi_callback_info info) {
+    size_t argc = 2; napi_value argv[2];
+    NAPI_OK(napi_get_cb_info(env, info, &argc, argv, nullptr, nullptr));
+    bb_backend* b = BackendOf(env, argv[0]); if (!b) return Throw(env, BB_ERR_ARG);
+    uint32_t which = 0; NAPI_OK(napi_get_value_uint32(env, argv[1], &which));
+    bb_query_log_records r;
+    const int rc = bb_query_log_backend(b, (int)std::min(which, 2u), &r);
+    return rc == BB_OK ? QueryLogObject(env, r) : Throw(env, rc);
 }
 static napi_value BackendDestroy(napi_env env, napi_callback_info info) {
     size_t argc = 1; napi_value argv[1];
@@ -540,10 +604,14 @@ static napi_value Init(napi_env env, napi_value exports) {
         { "tcpHubClose", nullptr, TcpHubClose, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "tcpHubRelay", nullptr, TcpHubRelay, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "tcpHubStats", nullptr, TcpHubStats, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubSetQueryLog", nullptr, TcpHubSetQueryLog, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "tcpHubQueryLog", nullptr, TcpHubQueryLog, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "backendCreate", nullptr, BackendCreate, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "backendFeed", nullptr, BackendFeed, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "backendRelay", nullptr, BackendRelay, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "backendStats", nullptr, BackendStats, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "backendSetQueryLog", nullptr, BackendSetQueryLog, nullptr, nullptr, nullptr, napi_default, nullptr },
+        { "backendQueryLog", nullptr, BackendQueryLog, nullptr, nullptr, nullptr, napi_default, nullptr },
         { "backendDestroy", nullptr, BackendDestroy, nullptr, nullptr, nullptr, napi_default, nullptr },
     };
     napi_define_properties(env, exports, sizeof d / sizeof d[0], d);

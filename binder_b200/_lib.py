@@ -93,6 +93,8 @@ SYMBOLS = {
     'bb_backend_feed': (_c.c_int, [_c.c_void_p, _c.c_void_p, _c.c_size_t, _c.c_uint64, _c.c_void_p, _c.c_void_p, _c.c_void_p]),
     'bb_backend_relay': (_c.c_int, [_c.c_void_p] * 7 + [_c.c_uint32, _c.c_void_p, _c.c_void_p]),
     'bb_backend_stat': (_c.c_uint64, [_c.c_void_p, _c.c_int]),
+    'bb_query_log_backend_enable': (_c.c_int, [_c.c_void_p, _c.c_int]),
+    'bb_query_log_backend': (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p]),
     'bb_tcp_hub_create': (_c.c_void_p, [_c.c_void_p, _c.c_uint32, _c.POINTER(_c.c_int)]),
     'bb_tcp_hub_destroy': (None, [_c.c_void_p]),
     'bb_tcp_hub_open': (_c.c_int, [_c.c_void_p, _c.c_void_p]),
@@ -105,6 +107,8 @@ SYMBOLS = {
     'bb_tcp_hub_relay': (_c.c_int, [_c.c_void_p] * 6 + [_c.c_uint32]),
     'bb_tcp_hub_peer': (_c.c_int, [_c.c_void_p, _c.c_uint32, _c.c_void_p, _c.c_void_p]),
     'bb_tcp_hub_stat': (_c.c_uint64, [_c.c_void_p, _c.c_int]),
+    'bb_query_log_tcp_hub_enable': (_c.c_int, [_c.c_void_p, _c.c_int]),
+    'bb_query_log_tcp_hub': (_c.c_int, [_c.c_void_p, _c.c_int, _c.c_void_p]),
     'bb_host_alloc': (_c.c_void_p, [_c.c_size_t]),
     'bb_host_free': (None, [_c.c_void_p]),
 }

@@ -23,10 +23,12 @@ Misses (lib/server.js:110-113,222-225) go to the recursion with the owner's sink
 its own with the source address as the tag and relays what its sink drains into OUTBOUND_UDP frames (relay(), UDP size
 limits); a hub's host submits flush()'s misses with the session id as the tag and hands what it drains to hub.relay().
 """
+import ctypes
 import struct
 
 import numpy as np
 
+from .query_log import QueryLogRecords
 from .recursion import QueueSink, split_packets
 from .server import TcpFramer, pack_packets
 
@@ -98,14 +100,92 @@ def build_frames(out, out_off, out_len, status, dst_ip, dst_port, control=()):
     return ctrl + buf.tobytes()
 
 
-class Backend(object):
+class _LogSet(object):
+    """The query-log records of a Python session's last call of one kind, as the native sessions keep them (bb_log_set,
+    csrc/balancer_backend.h): one resolver.log_batch per batch with an answer, a record per answer sent, in send order."""
+
+    def __init__(self):
+        self.on, self.records, self.lost = False, 0, 0
+        self.clear()
+
+    def clear(self):
+        self.logs, self.rows, self.used, self.call_lost = [], [], 0, 0
+
+    def batch(self, resolver, out, out_off, out_len, status, sent):
+        """sent: [(i, ip, port, session)] of the answered responses sent, in send order."""
+        if not self.on or not (np.asarray(status) == 0).any():
+            return
+        try:
+            log, log_off, log_len, head_len = resolver.log_batch(out, out_off, out_len, status)
+        except Exception:                            # BinderError: the answers are sent anyway, their records are lost
+            self.call_lost += len(sent)
+            self.lost += len(sent)
+            return
+        out = np.asarray(out)
+        for i, ip, port, sid in sent:
+            r = int(out_off[i])
+            req_id = (int(out[r]) << 8) | int(out[r + 1]) if int(out_len[i]) >= 2 else 0
+            self.rows.append((self.used + int(log_off[i]), int(log_len[i]), int(head_len[i]), req_id, ip, port, sid))
+        self.logs.append(np.asarray(log, dtype=np.uint8))
+        self.used += len(log)
+        self.records += len(sent)
+
+    def result(self, with_session):
+        rows = self.rows
+        col = lambda k, dt: np.array([r[k] for r in rows], dtype=dt)
+        log = np.concatenate(self.logs) if self.logs else np.zeros(0, np.uint8)
+        return QueryLogRecords(log, col(0, np.uint32), col(1, np.uint32), col(2, np.uint16), col(3, np.uint16), col(4, np.uint32),
+                               col(5, np.uint32), col(6, np.uint32) if with_session else None, self.call_lost)
+
+
+class _QueryLogging(object):
+    """set_query_log / query_log of the Python sessions: _log = (last feed or flush, last relay)."""
+    _with_session = False
+
+    def set_query_log(self, on):
+        for ls in self._log:
+            ls.on = bool(on)
+            ls.clear()
+
+    def query_log(self, which):
+        return self._log[which].result(self._with_session)
+
+    def _count_log(self):
+        self.counters['records'] = sum(ls.records for ls in self._log)
+        self.counters['lost'] = sum(ls.lost for ls in self._log)
+
+
+def _native_records(L, fn, h, which, with_session):
+    """bb_query_log_backend / bb_query_log_tcp_hub -> QueryLogRecords of numpy copies"""
+    from ._lib import check
+    P = ctypes.POINTER
+
+    class Records(ctypes.Structure):
+        _fields_ = [('n', ctypes.c_uint32), ('log', P(ctypes.c_uint8)), ('log_off', P(ctypes.c_uint32)), ('log_len', P(ctypes.c_uint32)),
+                    ('head_len', P(ctypes.c_uint16)), ('req_id', P(ctypes.c_uint16)), ('client_ip', P(ctypes.c_uint32)),
+                    ('client_port', P(ctypes.c_uint32)), ('session', P(ctypes.c_uint32)), ('lost', ctypes.c_uint32)]
+    if not h:
+        check(-1)
+    r = Records()
+    check(getattr(L, fn)(h, which, ctypes.byref(r)))
+    n = r.n
+    arr = lambda p, dt: np.ctypeslib.as_array(p, (n,)).astype(dt) if n else np.zeros(0, dt)
+    off, ln = arr(r.log_off, np.uint32), arr(r.log_len, np.uint32)
+    end = int((off.astype(np.int64) + ln).max()) if n else 0
+    log = np.ctypeslib.as_array(r.log, (end,)).copy() if end else np.zeros(0, np.uint8)
+    return QueryLogRecords(log, off, ln, arr(r.head_len, np.uint16), arr(r.req_id, np.uint16), arr(r.client_ip, np.uint32),
+                           arr(r.client_port, np.uint32), arr(r.session, np.uint32) if with_session else None, int(r.lost))
+
+
+class Backend(_QueryLogging):
     """One balancer session: feed() bytes read from the AF_UNIX socket, get bytes to write back.
 
     With a recursion, feed() submits every miss with this session's sink (a QueueSink that calls `wake`, from the
     recursion thread, when a window arrives) and the source (ip, port) as the tag; drain() then returns the OUTBOUND_UDP
     frames of the relays that arrived.  relay(queries, upstreams, dst) builds them on `relayer` (anything with
     relay_batch; the resolver by default) in batches of max_batch, as NativeBackend.relay (bb_backend_relay) does: a
-    failed batch gets no frames and is counted."""
+    failed batch gets no frames and is counted.  set_query_log(True): each batch's answers also get their "DNS query"
+    log records (the resolver's or relayer's log_batch), read with query_log(0: last feed, 1: last relay)."""
 
     def __init__(self, resolver, recursion=None, shuffle_seed=1, relayer=None, max_batch=1 << 14, wake=None):
         self.resolver, self.recursion, self.seed = resolver, recursion, shuffle_seed
@@ -113,9 +193,11 @@ class Backend(object):
         self.max_batch = max_batch
         self.sink = QueueSink(wake)
         self.pending = b''
-        self.counters = {'udp': 0, 'answered': 0, 'missed': 0, 'dropped': 0, 'relayed': 0, 'relay_failed': 0}
+        self.counters = {'udp': 0, 'answered': 0, 'missed': 0, 'dropped': 0, 'relayed': 0, 'relay_failed': 0, 'records': 0, 'lost': 0}
+        self._log = (_LogSet(), _LogSet())
 
     def feed(self, chunk):
+        self._log[0].clear()
         self.pending += bytes(chunk)
         data, off, ips, ports, control, used = parse_frames(self.pending)
         self.pending = self.pending[used:]
@@ -126,6 +208,9 @@ class Backend(object):
         out, out_off, out_len, status, miss = self.resolver.resolve_batch(data, off, seed=self.seed, qidx_base=0)
         c = self.counters
         c['udp'] += n; c['answered'] += int((status == 0).sum()); c['missed'] += len(miss); c['dropped'] += int((status == 2).sum())
+        self._log[0].batch(self.resolver, out, out_off, out_len, status,
+                           [(i, int(ips[i]), int(ports[i]), 0) for i in np.flatnonzero(status == 0)])
+        self._count_log()
         if self.recursion is not None:
             for i in miss:
                 i = int(i)
@@ -136,6 +221,7 @@ class Backend(object):
         """Replies to misses (query i answered from upstream response i, b'' = the lookup failed) -> bytes of one
         OUTBOUND_UDP frame per answered reply, addressed to dst[i] = (ip, port)."""
         c, frames = self.counters, []
+        self._log[1].clear()
         for k0 in range(0, len(queries), self.max_batch):
             qs, us, ds = queries[k0:k0 + self.max_batch], upstreams[k0:k0 + self.max_batch], dst[k0:k0 + self.max_batch]
             try:
@@ -144,6 +230,9 @@ class Backend(object):
                 c['relay_failed'] += len(qs)
                 continue
             c['relayed'] += int((np.asarray(status) == 0).sum())
+            self._log[1].batch(self.relayer, out, out_off, out_len, status,
+                               [(j, ds[j][0], ds[j][1], 0) for j in np.flatnonzero(np.asarray(status) == 0)])
+            self._count_log()
             frames.append(build_frames(out, out_off, out_len, status, [ip for ip, _ in ds], [p for _, p in ds]))
         return b''.join(frames)
 
@@ -188,7 +277,9 @@ def build_frames_native(out, out_off, out_len, status, dst_ip, dst_port, control
 
 
 class NativeBackend(object):
-    """bb_backend: one balancer session in the C library (frames in -> bb_resolve_batch -> frames out)."""
+    """bb_backend: one balancer session in the C library (frames in -> bb_resolve_batch -> frames out).
+    set_query_log(True) turns on the "DNS query" log records of its answers; query_log(0: last feed, 1: last relay)
+    returns them as a QueryLogRecords of numpy copies."""
 
     def __init__(self, engine, max_batch=1 << 14, lib=None):
         import ctypes
@@ -235,8 +326,15 @@ class NativeBackend(object):
         self.last_rc = rc
         return ctypes.string_at(out, out_len.value) if out_len.value else b''
 
+    def set_query_log(self, on):
+        from ._lib import check
+        check(self._L.bb_query_log_backend_enable(self._h, 1 if on else 0) if self._h else -1)
+
+    def query_log(self, which):
+        return _native_records(self._L, 'bb_query_log_backend', self._h, which, False)
+
     def stats(self):
-        keys = ('udp', 'answered', 'missed', 'dropped', 'pending_bytes', 'failed', 'relayed', 'relay_failed')
+        keys = ('udp', 'answered', 'missed', 'dropped', 'pending_bytes', 'failed', 'relayed', 'relay_failed', 'records', 'lost')
         return {k: int(self._L.bb_backend_stat(self._h, i)) for i, k in enumerate(keys)}
 
     def close(self):
@@ -264,14 +362,17 @@ class _TcpSession(object):
         self.queued = self.relays = self.ip = self.port = 0
 
 
-class TcpHub(object):
+class TcpHub(_QueryLogging):
     """The TCP hub (bb_tcp_hub, include/binder_b200.h) in Python, around an injected resolver (Engine or the CPU oracle)
     and relayer (anything with relay_batch(q_data, q_off, up_data, up_off, tcp=True); the resolver by default).
 
     open() -> session id; feed(id, bytes) -> False on a protocol error; eof(id); flush(seed) -> [(miss packet, id)];
     output(id) -> (bytes to write, closable); consume(id, n); close(id); relay(queries, upstreams, ids).  Limits as the
     native hub's: max_batch queries and max_batch_bytes query bytes per batch, out_cap answer bytes per batch (None: the
-    resolver's own limit).  A batch the resolver fails, or whose answers exceed out_cap, loses its queries (counted)."""
+    resolver's own limit).  A batch the resolver fails, or whose answers exceed out_cap, loses its queries (counted).
+    set_query_log(True) / query_log(0: last flush, 1: last relay): the answers' "DNS query" log records, as the native
+    hub keeps them (the resolver's and relayer's log_batch)."""
+    _with_session = True
 
     def __init__(self, resolver, max_batch=4096, max_batch_bytes=None, out_cap=None, relayer=None):
         self.resolver, self.relayer = resolver, relayer if relayer is not None else resolver
@@ -279,7 +380,8 @@ class TcpHub(object):
         self.max_bytes = max_batch_bytes if max_batch_bytes is not None else max(64 * max_batch, 1 << 16)
         self.out_cap = out_cap
         self.sessions, self.next_id, self.queue = {}, 1, []
-        self.counters = dict.fromkeys(HUB_STATS[:8], 0)
+        self.counters = dict.fromkeys(HUB_STATS[:8] + ('records', 'lost'), 0)
+        self._log = (_LogSet(), _LogSet())
 
     def _get(self, sid):
         s = self.sessions.get(sid)
@@ -341,6 +443,7 @@ class TcpHub(object):
 
     def flush(self, seed):
         queue, self.queue, c = self.queue, [], self.counters
+        self._log[0].clear()
         misses, qidx, i = [], 0, 0
         while i < len(queue):
             batch, nbytes = [], 0
@@ -369,6 +472,9 @@ class TcpHub(object):
                 c['failed'] += len(batch)
                 continue
             out, out_off, out_len, status, _ = res
+            self._log[0].batch(self.resolver, out, out_off, out_len, status,
+                               [(k, self.sessions[sid].ip, self.sessions[sid].port, sid) for k, (_, sid) in enumerate(batch) if status[k] == 0])
+            self._count_log()
             for k, (m, sid) in enumerate(batch):
                 s = self.sessions[sid]
                 if status[k] == 0:
@@ -385,9 +491,14 @@ class TcpHub(object):
     def relay(self, queries, upstreams, sids):
         """Replies to misses: query i answered from upstream response i (b'' = the lookup failed), appended to sids[i]."""
         c = self.counters
+        self._log[1].clear()
         for k0 in range(0, len(sids), self.max_batch):
             qs, us, ss = queries[k0:k0 + self.max_batch], upstreams[k0:k0 + self.max_batch], sids[k0:k0 + self.max_batch]
             res = self._answers(self.relayer.relay_batch, *(pack_packets(qs) + pack_packets(us)))
+            if res is not None:
+                live = [(j, self.sessions.get(sid), sid) for j, sid in enumerate(ss) if res[3][j] == 0]
+                self._log[1].batch(self.relayer, *res, [(j, s.ip, s.port, sid) for j, s, sid in live if s is not None])
+                self._count_log()
             for j, sid in enumerate(ss):
                 s = self.sessions.get(sid)
                 if s is not None and s.relays:
@@ -426,7 +537,8 @@ class TcpHub(object):
 class NativeTcpHub(object):
     """bb_tcp_hub: TCP proxy sessions in the C library, their messages resolved as TCP batches on the engine.  Same
     methods as TcpHub; argument errors (unknown or closed session, a closed hub) raise BinderError.  A failed batch is
-    counted, not raised: its code is in last_rc.  `lib` is the library to call (libbinder_b200.so by default)."""
+    counted, not raised: its code is in last_rc.  `lib` is the library to call (libbinder_b200.so by default).
+    query_log(which) returns the records as a QueryLogRecords of numpy copies."""
 
     def __init__(self, engine, max_batch=4096, lib=None):
         import ctypes
@@ -508,7 +620,16 @@ class NativeTcpHub(object):
     def stats(self):
         st = {k: int(self._L.bb_tcp_hub_stat(self._h, i)) for i, k in enumerate(HUB_STATS)}
         st['answer_capacity'] = int(self._L.bb_tcp_hub_stat(self._h, len(HUB_STATS)))
+        st['records'] = int(self._L.bb_tcp_hub_stat(self._h, len(HUB_STATS) + 1))
+        st['lost'] = int(self._L.bb_tcp_hub_stat(self._h, len(HUB_STATS) + 2))
         return st
+
+    def set_query_log(self, on):
+        from ._lib import check
+        check(self._L.bb_query_log_tcp_hub_enable(self._h, 1 if on else 0) if self._h else -1)
+
+    def query_log(self, which):
+        return _native_records(self._L, 'bb_query_log_tcp_hub', self._h, which, True)
 
     def destroy(self):
         if getattr(self, '_h', None):

@@ -9,7 +9,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 SO = os.path.join(HERE, 'libbinder_b200.so')
 SRCS = [os.path.join(HERE, 'csrc', f) for f in ('engine.cu', 'zone_build.cpp', 'balancer_frames.cpp', 'balancer_relay.cpp',
-                                                'balancer_tcp.cpp')]
+                                                'balancer_tcp.cpp', 'balancer_query_log.cpp')]
 DEPS = SRCS + [os.path.join(HERE, 'csrc', 'zone_image.h'), os.path.join(HERE, 'csrc', 'resolve_device.cuh'),
                os.path.join(HERE, 'csrc', 'balancer_backend.h'), os.path.join(HERE, 'csrc', 'relay_device.cuh'), os.path.join(HERE, 'csrc', 'log_device.cuh'),
                os.path.join(HERE, 'csrc', 'forward_device.cuh'),

@@ -95,6 +95,7 @@ bb_backend* bb_backend_create(bb_engine* e, uint32_t max_batch, int* err) {
         bb_backend_destroy(b); if (err) *err = BB_ERR_NOMEM; return nullptr;
     }
     memset(b->pkts, 0, b->max_bytes + 64);
+    b->qlog[0].max_batch = b->qlog[1].max_batch = max_batch;
     return b;
 }
 
@@ -102,6 +103,7 @@ void bb_backend_destroy(bb_backend* b) {
     if (!b) return;
     bb_host_free(b->pkts); bb_host_free(b->pkt_off); bb_host_free(b->ip); bb_host_free(b->port); bb_host_free(b->resp);
     bb_host_free(b->resp_off); bb_host_free(b->resp_len); bb_host_free(b->status); bb_host_free(b->miss);
+    b->qlog[0].release(); b->qlog[1].release();
     delete b;
 }
 
@@ -109,7 +111,7 @@ int bb_backend_feed(bb_backend* b, const uint8_t* in, size_t in_len, uint64_t sh
                     const uint8_t** out, size_t* out_len, bb_backend_misses* misses) {
     if (!b || (!in && in_len) || !out || !out_len) return BB_ERR_ARG;
     b->pending.insert(b->pending.end(), in, in + in_len);
-    b->out.clear(); b->m_pkts.clear(); b->m_off.assign(1, 0); b->m_ip.clear(); b->m_port.clear();
+    b->out.clear(); b->m_pkts.clear(); b->m_off.assign(1, 0); b->m_ip.clear(); b->m_port.clear(); b->qlog[0].clear();
     size_t pos = 0; int rc = BB_OK;
     b->qidx_next = 0;                                   // (seed, index) keys the shuffle: indices run over the queries of this feed
     for (;;) {
@@ -135,6 +137,10 @@ int bb_backend_feed(bb_backend* b, const uint8_t* in, size_t in_len, uint64_t sh
                 if (need) bb_frames_build(b->resp, b->resp_off, b->resp_len, b->status, b->ip, b->port, 0, control, nc, b->out.data() + at, need, &need);
                 break;
             }
+            // record i of the batch goes with its OUTBOUND_UDP frame, which bb_frames_build below writes in index order
+            b->qlog[0].batch(b->e, b->resp, b->resp_off, b->resp_len, b->status, n, [b](uint32_t i, uint32_t& ip, uint32_t& port, uint32_t&) {
+                ip = b->ip[i]; port = b->port[i]; return true;
+            });
             b->n_udp += n; b->n_missed += n_miss;
             for (uint32_t i = 0; i < n; i++) { b->n_answered += b->status[i] == BB_ANSWERED; b->n_dropped += b->status[i] == BB_DROPPED; }
             for (uint32_t k = 0; k < n_miss; k++) {                     // lib/server.js:110-113,222-225: these go to recursion
@@ -162,7 +168,8 @@ int bb_backend_feed(bb_backend* b, const uint8_t* in, size_t in_len, uint64_t sh
 uint64_t bb_backend_stat(const bb_backend* b, int what) {
     if (!b) return 0;
     switch (what) { case 0: return b->n_udp; case 1: return b->n_answered; case 2: return b->n_missed; case 3: return b->n_dropped; case 4: return b->pending.size(); case 5: return b->n_failed;
-                    case 6: return b->n_relayed; case 7: return b->n_relay_failed; }
+                    case 6: return b->n_relayed; case 7: return b->n_relay_failed;
+                    case 8: return b->qlog[0].n_records + b->qlog[1].n_records; case 9: return b->qlog[0].n_lost + b->qlog[1].n_lost; }
     return 0;
 }
 

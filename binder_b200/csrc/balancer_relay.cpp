@@ -11,7 +11,7 @@ extern "C" {
 int bb_backend_relay(bb_backend* b, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* up_pkts, const uint32_t* up_off,
                      const uint32_t* dst_ip, const uint32_t* dst_port, uint32_t n, const uint8_t** out, size_t* out_len) {
     if (!b || !out || !out_len) return BB_ERR_ARG;
-    b->r_out.clear();
+    b->r_out.clear(); b->qlog[1].clear();
     *out = b->r_out.data(); *out_len = 0;
     if (n == 0) return BB_OK;
     if (!q_off || !up_off || !dst_ip || !dst_port || (q_off[n] != q_off[0] && !q_pkts) || (up_off[n] != up_off[0] && !up_pkts))
@@ -29,6 +29,9 @@ int bb_backend_relay(bb_backend* b, const uint8_t* q_pkts, const uint32_t* q_off
             b->n_relay_failed += m;
             continue;
         }
+        b->qlog[1].batch(b->e, b->resp, b->resp_off, b->resp_len, b->status, m, [&](uint32_t j, uint32_t& ip, uint32_t& port, uint32_t&) {
+            ip = dst_ip[k0 + j]; port = dst_port[k0 + j]; return true;
+        });
         size_t need = 0;
         bb_frames_build(b->resp, b->resp_off, b->resp_len, b->status, dst_ip + k0, dst_port + k0, m, nullptr, 0, nullptr, 0, &need);
         const size_t at = b->r_out.size();

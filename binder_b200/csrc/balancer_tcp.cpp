@@ -6,7 +6,7 @@
 // holds many such sessions of one engine: feed() de-frames each session's bytes into one queue, flush() resolves the
 // whole queue as TCP batches (bb_resolve_batch_ex with BB_BATCH_TCP) and appends each answer, length-prefixed, to its
 // session's output.  The host keeps the sockets.  Host code only: no CUDA in this file.
-#include "../../include/binder_b200.h"
+#include "balancer_backend.h"                          // bb_log_set: the query-log records
 
 #include <algorithm>
 #include <cstring>
@@ -44,9 +44,12 @@ struct bb_tcp_hub {
     std::vector<uint8_t> m_pkts; std::vector<uint32_t> m_off, m_sid;    // misses of the last flush
     std::vector<uint32_t> r_qoff, r_upoff;             // a relay batch's offsets, rebased
     uint64_t n_sessions = 0, n_msgs = 0, n_answered = 0, n_missed = 0, n_dropped = 0, n_proto = 0, n_failed = 0, n_relayed = 0;
+    bb_log_set qlog[2];                                // query-log records of the last flush [0] and the last relay [1]
 
     TcpSession* find(uint32_t id) { auto it = sess.find(id); return it == sess.end() ? nullptr : &it->second; }
 };
+
+bb_log_set* tcp_hub_log_sets(bb_tcp_hub* h) { return h->qlog; }
 
 extern "C" {
 
@@ -70,6 +73,7 @@ bb_tcp_hub* bb_tcp_hub_create(bb_engine* e, uint32_t max_batch, int* err) {
     }
     memset(h->pkts, 0, (size_t)h->max_bytes + 64);
     h->b_sid.resize(max_batch);
+    h->qlog[0].max_batch = h->qlog[1].max_batch = max_batch;
     return h;
 }
 
@@ -77,6 +81,7 @@ void bb_tcp_hub_destroy(bb_tcp_hub* h) {
     if (!h) return;
     bb_host_free(h->pkts); bb_host_free(h->pkt_off); bb_host_free(h->resp); bb_host_free(h->resp_off);
     bb_host_free(h->resp_len); bb_host_free(h->status); bb_host_free(h->miss);
+    h->qlog[0].release(); h->qlog[1].release();
     delete h;
 }
 
@@ -135,7 +140,7 @@ int bb_tcp_hub_eof(bb_tcp_hub* h, uint32_t session) {
 
 int bb_tcp_hub_flush(bb_tcp_hub* h, uint64_t shuffle_seed, bb_tcp_hub_misses* misses) {
     if (!h) return BB_ERR_ARG;
-    h->m_pkts.clear(); h->m_off.assign(1, 0); h->m_sid.clear();
+    h->m_pkts.clear(); h->m_off.assign(1, 0); h->m_sid.clear(); h->qlog[0].clear();
     const size_t total = h->q_sid.size();
     int rc = BB_OK;
     uint32_t qidx = 0;                                 // (seed, qidx) keys the service shuffle: it does not repeat across batches
@@ -164,6 +169,11 @@ int bb_tcp_hub_flush(bb_tcp_hub* h, uint64_t shuffle_seed, bb_tcp_hub_misses* mi
             for (uint32_t k = 0; k < n; k++) h->find(h->b_sid[k])->queued--;
             continue;
         }
+        // the answers are appended below in query order, each to the session that asked
+        h->qlog[0].batch(h->e, h->resp, h->resp_off, h->resp_len, h->status, n, [h](uint32_t k, uint32_t& ip, uint32_t& port, uint32_t& sid) {
+            const TcpSession* s = h->find(h->b_sid[k]);
+            ip = s->ip; port = s->port; sid = h->b_sid[k]; return true;
+        });
         // per session in arrival order; misses in query order whatever the packing
         TcpSession* s = nullptr; uint32_t sid = 0;
         for (uint32_t k = 0; k < n; k++) {
@@ -216,6 +226,7 @@ int bb_tcp_hub_close(bb_tcp_hub* h, uint32_t session) {
 int bb_tcp_hub_relay(bb_tcp_hub* h, const uint8_t* q_pkts, const uint32_t* q_off, const uint8_t* up_pkts,
                      const uint32_t* up_off, const uint32_t* sessions, uint32_t n) {
     if (!h) return BB_ERR_ARG;
+    h->qlog[1].clear();
     if (n == 0) return BB_OK;
     if (!q_off || !up_off || !sessions || (q_off[n] != q_off[0] && !q_pkts) || (up_off[n] != up_off[0] && !up_pkts)) return BB_ERR_ARG;
     for (uint32_t i = 0; i < n; i++) if (q_off[i + 1] < q_off[i] || up_off[i + 1] < up_off[i]) return BB_ERR_ARG;
@@ -226,6 +237,13 @@ int bb_tcp_hub_relay(bb_tcp_hub* h, const uint8_t* q_pkts, const uint32_t* q_off
         for (uint32_t j = 0; j <= m; j++) { h->r_qoff[j] = q_off[k0 + j] - q_off[k0]; h->r_upoff[j] = up_off[k0 + j] - up_off[k0]; }
         const int r = bb_relay_batch(h->e, q_pkts ? q_pkts + q_off[k0] : nullptr, h->r_qoff.data(), up_pkts ? up_pkts + up_off[k0] : nullptr,
                                      h->r_upoff.data(), m, BB_BATCH_TCP, h->resp, h->resp_cap, h->resp_off, h->resp_len, h->status);
+        // a reply is appended (and has a record) when its session is still open
+        if (r == BB_OK)
+            h->qlog[1].batch(h->e, h->resp, h->resp_off, h->resp_len, h->status, m, [&](uint32_t j, uint32_t& ip, uint32_t& port, uint32_t& sid) {
+                const TcpSession* s = h->find(sessions[k0 + j]);
+                if (!s) return false;
+                ip = s->ip; port = s->port; sid = sessions[k0 + j]; return true;
+            });
         for (uint32_t j = 0; j < m; j++) {
             TcpSession* s = h->find(sessions[k0 + j]);
             if (s && s->relays) s->relays--;
@@ -253,6 +271,7 @@ uint64_t bb_tcp_hub_stat(const bb_tcp_hub* h, int what) {
     case 0: return h->n_sessions; case 1: return h->n_msgs; case 2: return h->n_answered; case 3: return h->n_missed;
     case 4: return h->n_dropped; case 5: return h->n_proto; case 6: return h->n_failed; case 7: return h->n_relayed;
     case 8: return h->sess.size(); case 9: return h->q_sid.size(); case 10: return h->resp_cap;
+    case 11: return h->qlog[0].n_records + h->qlog[1].n_records; case 12: return h->qlog[0].n_lost + h->qlog[1].n_lost;
     }
     return 0;
 }

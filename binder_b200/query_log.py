@@ -8,7 +8,10 @@ bunyan and the handler add around them, in bunyan's order:
    "level":30|40,<body>,"latency":<ms>,"timers":{},"msg":"DNS query","time":<ISO 8601>,"v":0}
 
 One line per record, newline-terminated, UTF-8.  level is 40 (warn) when the latency is over 1,000 ms (:511-514).
+write() renders a batch's records and writes their lines; write_records() writes the lines of the records a balancer
+session kept of its last call (QueryLogRecords: NativeBackend / NativeTcpHub.query_log and their Python models).
 """
+import collections
 import json
 import os
 import socket
@@ -16,6 +19,16 @@ import threading
 import time
 
 import numpy as np
+
+# The records of a balancer session's last call (bb_query_log_records): record i = log[log_off[i]:log_off[i] + log_len[i]],
+# its first head_len[i] bytes the head fragment; req_id, client_ip (IPv4 as a u32, 127.0.0.1 = 0x7F000001), client_port
+# and, for a TCP hub, session per record (None for a UDP backend); lost = answers whose log call failed.
+QueryLogRecords = collections.namedtuple('QueryLogRecords', 'log log_off log_len head_len req_id client_ip client_port session lost')
+
+
+def ipv4_text(ip):
+    ip = int(ip)
+    return '%d.%d.%d.%d' % (ip >> 24, (ip >> 16) & 255, (ip >> 8) & 255, ip & 255)
 
 
 def iso_time(t):
@@ -54,16 +67,35 @@ class QueryLog(object):
         out = np.asarray(out)
         parts = []
         for i in np.flatnonzero(log_len):
-            o, hl, ll = int(log_off[i]), int(head_len[i]), int(log_len[i])
             r = int(out_off[i])
-            req_id = (int(out[r]) << 8) | int(out[r + 1])
-            addr, port = clients[i][0], clients[i][1]
-            lat = max(0, int((sent - received[i]) * 1000))
-            parts.append(b''.join((
-                ('%s"req_id":%d,"client":%s,"port":"%d/%s",' % (self._prefix, req_id, json.dumps(addr), port,
-                                                                'ipv6' if ':' in addr else 'ipv4')).encode(),
-                log[o:o + hl], b',"level":%d,' % (40 if lat > 1000 else 30), log[o + hl:o + ll],
-                (',"latency":%d,"timers":{},"msg":"DNS query","time":"%s","v":0}\n' % (lat, stamp)).encode())))
+            parts.append(self._line((int(out[r]) << 8) | int(out[r + 1]), clients[i][0], clients[i][1], log, int(log_off[i]),
+                                    int(head_len[i]), int(log_len[i]), sent - received[i], stamp))
+        return self._emit(parts)
+
+    def write_records(self, records, received, sent=None):
+        """The lines of a balancer session's records (a QueryLogRecords), client "a.b.c.d", port "<port>/ipv4".
+        received: when each record's query arrived (time.time(); one value for all, or one per record).  sent: when
+        the answers went out (default: now).  A record that is empty (its response did not decode) has no line."""
+        n = len(records.log_len)
+        received = np.broadcast_to(np.asarray(received, dtype=np.float64), (n,))
+        sent = time.time() if sent is None else sent
+        stamp = iso_time(sent)
+        log = np.asarray(records.log, dtype=np.uint8).tobytes()
+        parts = [self._line(int(records.req_id[i]), ipv4_text(records.client_ip[i]), int(records.client_port[i]), log,
+                            int(records.log_off[i]), int(records.head_len[i]), int(records.log_len[i]), sent - received[i], stamp)
+                 for i in np.flatnonzero(records.log_len)]
+        return self._emit(parts)
+
+    def _line(self, req_id, addr, port, log, o, hl, ll, wait, stamp):
+        """One line: the record log[o:o + ll] (head: its first hl bytes), `wait` seconds after its query arrived."""
+        lat = max(0, int(wait * 1000))
+        return b''.join((
+            ('%s"req_id":%d,"client":%s,"port":"%d/%s",' % (self._prefix, req_id, json.dumps(addr), port,
+                                                            'ipv6' if ':' in addr else 'ipv4')).encode(),
+            log[o:o + hl], b',"level":%d,' % (40 if lat > 1000 else 30), log[o + hl:o + ll],
+            (',"latency":%d,"timers":{},"msg":"DNS query","time":"%s","v":0}\n' % (lat, stamp)).encode()))
+
+    def _emit(self, parts):
         if parts:
             with self._lock:
                 self.stream.write(b''.join(parts))

@@ -483,6 +483,8 @@ int bb_shard_results(bb_shard* s, uint32_t src, const uint8_t** out, const uint3
  *                     (capacity, CUDA, an engine without `recursion`) loses its relays, counts them (stat 7) and the
  *                     call goes on with the next batch; the return value is then the first batch's error.  BB_ERR_ARG
  *                     for null arrays or decreasing offsets.
+ *   bb_query_log_backend_enable / bb_query_log_backend   binder's "DNS query" log records (lib/server.js:509-591) of the
+ *                     answers a session sends: see bb_query_log_records below.  Off by default; stats 8 and 9.
  */
 enum { BB_FRAME_CLIENT_HELLO = 1, BB_FRAME_INBOUND_UDP = 2, BB_FRAME_INBOUND_TCP = 3, BB_FRAME_CLIENT_HEARTBEAT = 4,
        BB_FRAME_SERVER_HELLO = 1001, BB_FRAME_OUTBOUND_UDP = 1002, BB_FRAME_INBOUND_TCP_OK = 1003, BB_FRAME_SERVER_HEARTBEAT = 1004 };
@@ -504,8 +506,41 @@ int         bb_backend_relay(bb_backend* b, const uint8_t* q_pkts, const uint32_
                              const uint32_t* up_off, const uint32_t* dst_ip, const uint32_t* dst_port, uint32_t n,
                              const uint8_t** out, size_t* out_len);
 /* 0 udp frames 1 answered 2 missed 3 dropped 4 pending bytes 5 queries of failed batches 6 replies relayed
- * 7 queries of failed relay batches */
+ * 7 queries of failed relay batches 8 query-log records 9 answers whose query-log call failed (lost records) */
 uint64_t    bb_backend_stat(const bb_backend* b, int what);
+
+/* ---- query log of the balancer sessions (DESIGN.md section 15) -------------------------------------------------------
+ * With the query log on, every resolve or relay batch a session (bb_backend, bb_tcp_hub) runs that succeeds and has an
+ * answer gets one bb_log_batch call over its own result set.  The records of one call (a feed or flush: which = 0; a
+ * relay: which = 1) share one pinned buffer of the session, written by the kernel in place: batch k's records start
+ * where batch k-1's end (rounded up to 16 bytes).  Record i = log[log_off[i] .. log_off[i] + log_len[i]), its first
+ * head_len[i] bytes the head fragment, the rest the body; an answer that does not decode has an empty record.  One
+ * record per answer sent, in the order the answers were written: a feed's OUTBOUND_UDP frames (control replies have no
+ * record), a backend relay's frames, a flush's answers across sessions in the order they were appended, a hub relay's
+ * replies that were appended (a reply to a session closed meanwhile is not sent and has no record).  The client is the
+ * query's INBOUND_UDP source, the relay's (dst_ip, dst_port), or the hub session's INBOUND_TCP peer.  The records stay
+ * valid until the next call of the same kind: a feed does not invalidate the last relay's, nor a relay the last feed's.
+ * A log call that fails with BB_ERR_CAPACITY grows the buffer and runs once more; a batch whose log call still fails
+ * keeps its answers (they are sent), and they count in `lost` and in the lost-records stat.  The query log never
+ * changes a call's frames, outputs, misses, other stats or return code.
+ *   ..._enable      enable != 0: on (allocates the buffers; BB_ERR_NOMEM); 0: off (frees them; no records, no calls).
+ *   bb_query_log_backend / bb_query_log_tcp_hub   the records of the last call of kind `which`; n = 0 with the log off.
+ *                   BB_ERR_ARG for which > 1.
+ */
+typedef struct bb_query_log_records {
+    uint32_t n;                  /* records */
+    const uint8_t*  log;         /* the call's record bytes */
+    const uint32_t* log_off;     /* n: record i = log[log_off[i] .. log_off[i] + log_len[i]) */
+    const uint32_t* log_len;     /* n */
+    const uint16_t* head_len;    /* n: the first head_len[i] bytes are the head fragment */
+    const uint16_t* req_id;      /* n: the response's DNS ID */
+    const uint32_t* client_ip;   /* n: IPv4 as the frame carries it (127.0.0.1 = 0x7F000001) */
+    const uint32_t* client_port; /* n */
+    const uint32_t* session;     /* n for a hub: the record's session id; NULL for a backend */
+    uint32_t lost;               /* answered responses of the call whose log call failed */
+} bb_query_log_records;
+int         bb_query_log_backend_enable(bb_backend* b, int enable);
+int         bb_query_log_backend(const bb_backend* b, int which /* 0: last feed, 1: last relay */, bb_query_log_records* r);
 
 /* ---- mname-balancer TCP proxy sessions (deps/mname-balancer/backend.c:22-113, tcp_proxy.c:160-300) ----------------
  * The balancer hands every DNS-over-TCP client connection to a backend as its own AF_UNIX session.  The session opens
@@ -537,6 +572,9 @@ uint64_t    bb_backend_stat(const bb_backend* b, int what);
  *   relay    the host's upstream responses for misses (q = the miss packets, up = upstream i, empty = the lookup failed)
  *            through bb_relay_batch(BB_BATCH_TCP), each reply appended length-prefixed to sessions[i]: RFC 7766 allows
  *            out-of-order answers and the ID matches them.  Batches of max_batch; a failed one is counted as in flush.
+ *   bb_query_log_tcp_hub_enable / bb_query_log_tcp_hub   the "DNS query" log records of the answers appended by the last
+ *            flush (which = 0) or relay (which = 1), with each record's session id: bb_query_log_records above.  Off by
+ *            default; stats 11, 12.
  */
 typedef struct bb_tcp_hub bb_tcp_hub;
 typedef struct bb_tcp_hub_misses {
@@ -557,8 +595,10 @@ int         bb_tcp_hub_relay(bb_tcp_hub* h, const uint8_t* q_pkts, const uint32_
 int         bb_tcp_hub_peer(const bb_tcp_hub* h, uint32_t session, uint32_t* ip, uint32_t* port);
 /* 0 sessions opened 1 DNS messages received 2 answered 3 missed 4 dropped (undecodable, oversized, or of a closed session)
  * 5 protocol errors 6 queries of failed batches 7 relay replies appended 8 sessions open 9 messages queued for the next flush
- * 10 answer bytes per batch */
+ * 10 answer bytes per batch 11 query-log records 12 answers whose query-log call failed (lost records) */
 uint64_t    bb_tcp_hub_stat(const bb_tcp_hub* h, int what);
+int         bb_query_log_tcp_hub_enable(bb_tcp_hub* h, int enable);
+int         bb_query_log_tcp_hub(const bb_tcp_hub* h, int which /* 0: last flush, 1: last relay */, bb_query_log_records* r);
 
 /* pinned host memory for the batch containers */
 void* bb_host_alloc(size_t bytes);
